@@ -283,7 +283,9 @@ static int step_device(lgw_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, 
     a.tile_base = b0; a.chunk_lo = c0; a.chunk_hi = c1;
     a.seg_chunk = d_seg_chunk + s0; a.seg_slot = d_seg_slot + s0; a.n_segs = s1 - s0; a.out = d_out; a.seg_out = d_seg_out + s0;
     a.rowq = e->d_rowq; a.rowq_count = e->d_rowq_count; a.rowq_cap = e->lim.rowq_cap; a.s = e->scratch;
-    if (reset_rows) CK(e, cudaMemsetAsync(e->d_rowq_count, 0, 4, e->stream));
+    // the bulk path's first kernel empties the row queue; one call fewer on the host between the caller's enqueue and the kernels
+    a.reset_rows = reset_rows && e->mode == 0 && a.n_segs ? 1u : 0u;
+    if (reset_rows && !a.reset_rows) CK(e, cudaMemsetAsync(e->d_rowq_count, 0, 4, e->stream));
     int launched = 0;
     const bool pk = e->per_kernel_timing || e->mode == 1;
     cudaError_t r = launch_step(a, e->mode, e->sm_count, e->stream, e->ev, &launched, pk);

@@ -1218,6 +1218,7 @@ R2_GLOBAL void k_prime2(StepArgs a) {
     griddep_launch();
     const uint32_t i = R2_BID * R2_NTHR + R2_TID;
     if (i == 0) {
+        if (a.reset_rows) *a.rowq_count = 0;                                   // (the kernels after this one append rows)
         TemplateCache2* tc = a.s.tpl_cache2;
         uint32_t total = 0, full = 1, lo = 0;
         for (uint32_t s = 0; s < R2_SLOTS; ++s) { total += tc->hits[s]; if (tc->state[s] != 2u) full = 0; if (tc->hits[s] < tc->hits[lo]) lo = s; }
@@ -1259,8 +1260,11 @@ R2_GLOBAL void k_prime2(StepArgs a) {
 
 // ---- k_commit2 (one warp per segment) ----------------------------------------------------------------------------------------------
 #define R2_CWARPS 8u
-#ifndef R2_CBLOCKS                      /* resident blocks per SM the commit kernel is compiled for: 6 -> 40 registers, 4 -> 64, 3 -> 80 */
-#define R2_CBLOCKS 6
+#ifndef R2_CBLOCKS                      /* resident blocks per SM the commit kernel is compiled for: 6 -> 40 registers, 4 -> 64, 3 -> 80.
+                                           4 x 8 warps x 132 SMs hold a warp for each of C3's 4 096 segments at once, and with 64
+                                           registers ptxas reports 12 B of spill stores instead of 140 (DESIGN 4.3)
+                                           (3 blocks: two waves, no faster than 6; DESIGN 9.12) */
+#define R2_CBLOCKS 4
 #endif
 // the exact sequential machine over a stream's chunks (streams the bulk kernel could not vouch for), out of line
 R2_DEV_NOINLINE uint32_t commit_sequential(StepIO io, const uint8_t* data, const uint32_t* chunk_off, uint32_t c_from, uint32_t c_to, uint32_t emit_begin) {
@@ -1289,14 +1293,13 @@ struct TextReader {
     const uint8_t* text; uint32_t base, n;
     R2_MEM uint32_t at(uint32_t p) const { return p - base < n ? (uint32_t)text[p - base] : 0u; }
 };
-R2_DEV_NOINLINE void commit_usage_fields(const uint8_t* text, uint32_t ups, uint32_t ulen, uint32_t full_flags, const UsageRaw* tpl_raw, UsageRaw* raw, UsageRec* cand, uint32_t lane,
-                                         uint32_t f_start, uint32_t f_word) {
+R2_DEV_NOINLINE uint32_t commit_usage_fields(const uint8_t* text, uint32_t ups, uint32_t ulen, uint32_t full_flags, UsageRaw* raw, UsageRec* cand, uint32_t lane,
+                                             uint32_t f_start, uint32_t f_word) {
     TextReader rd{text, ups, ulen};
     const bool has_span = lane < 8u && f_word != 0xFFFFFFFFu;
     const uint32_t f_len = f_word & 0x7FFFFFFFu, f_esc = has_span ? f_word >> 31 : 0u;
     const uint32_t span_mask = __ballot_sync(R2_FULL, has_span);
     Val v; v.kind = KD_ABSENT; v.bits = 0;
-    for (uint32_t k = lane; k < sizeof(UsageRaw) / 4; k += 32) reinterpret_cast<uint32_t*>(raw)[k] = reinterpret_cast<const uint32_t*>(tpl_raw)[k];
     __syncwarp();
     const uint32_t slow_str = __ballot_sync(R2_FULL, has_span && lane >= UF_MODEL && f_esc != 0u);
     if (has_span) {
@@ -1317,10 +1320,11 @@ R2_DEV_NOINLINE void commit_usage_fields(const uint8_t* text, uint32_t ups, uint
             else if (fi == UF_COST) raw->cost = x; else if (fi == UF_REASONING) raw->reasoning = x; else raw->cached = x;
         }
     }
-    uint32_t has = 0;                                                                  // bit 0: the record carries "model" as a string, bit 1: "provider"
+    uint32_t has = 0, exotic = 0;                                                      // has bit 0: the record carries "model" as a string, bit 1: "provider"
     if (lane == 0) {
         normalise_usage(*raw, full_flags, *cand);
         has = (cand->model_val.kind == KD_STR ? 1u : 0u) | (cand->provider_val.kind == KD_STR ? 2u : 0u);
+        exotic = cand->exotic;
     }
     has = __shfl_sync(R2_FULL, has, 0);
     // plain strings (no escapes): the span's bytes ARE the decoded text -- copy them into the record, a lane per byte
@@ -1333,10 +1337,11 @@ R2_DEV_NOINLINE void commit_usage_fields(const uint8_t* text, uint32_t ups, uint
         for (uint32_t k = lane; k < n; k += 32) dst[k] = (char)rd.at(st + k);
         if (lane == 0) {
             if (which == 0) cand->model_len = (uint8_t)n; else cand->provider_len = (uint8_t)n;
-            if (ln > LGW_STR_CAP) { cand->str_flags |= which == 0 ? 1u : 4u; cand->exotic = 1; }      // truncated: reported, like the full machine's capture
+            if (ln > LGW_STR_CAP) { cand->str_flags |= which == 0 ? 1u : 4u; cand->exotic = 1; exotic = 1; }   // truncated: reported, like the full machine's capture
         }
     }
     __syncwarp();
+    return __shfl_sync(R2_FULL, exotic, 0);                                            // (the record's `exotic`, without reading it back)
 }
 
 R2_DEV_NOINLINE void commit_settle_pending(StepIO io) { resolve_pending(io); }
@@ -1346,20 +1351,8 @@ R2_DEV uint4 commit_ld16(const uint8_t* p) { return __ldg(reinterpret_cast<const
 R2_DEV uint4 commit_ld16(const uint8_t* p) { uint4 v; memcpy(&v, p, 16); return v; }
 #endif
 
-R2_GLOBAL void
-#if !R2_HOST_EMU
-__launch_bounds__(R2_CWARPS * 32, R2_CBLOCKS)      // (the full machine behind commit_usage_event / commit_sequential spills instead of costing every warp 142 registers)
-#endif
-k_commit2(StepArgs a) {
-#if !R2_HOST_EMU
-    __shared__ __align__(16) uint8_t stage[R2_CWARPS][LGW_PENDING_STRIDE];           // the winning usage event's text
-    __shared__ __align__(16) UsageRaw stage_raw[R2_CWARPS];                           // the record being assembled from it
-#else
-    alignas(16) static uint8_t stage[R2_CWARPS][LGW_PENDING_STRIDE];
-    static UsageRaw stage_raw[R2_CWARPS];
-#endif
-    const uint32_t seg = (R2_BID * R2_NTHR + R2_TID) >> 5, lane = R2_TID & 31u, warp = (R2_TID >> 5) % R2_CWARPS;
-    if (seg >= a.n_segs) return;
+// the commit of segment `seg` (one warp)
+R2_DEV void commit_one(const StepArgs& a, uint32_t seg, uint32_t lane, uint8_t* stage, UsageRaw* stage_raw, uint32_t* counts) {
     const uint32_t c0 = __ldg(a.seg_chunk + seg), c1 = __ldg(a.seg_chunk + seg + 1);
     const uint32_t slot = __ldg(a.seg_slot + seg);
     // Everything that does not depend on the bulk kernel runs BEFORE the wait, while that kernel is still at work (this kernel's
@@ -1380,6 +1373,7 @@ k_commit2(StepArgs a) {
     const bool any_empty = __any_sync(R2_FULL, empty);
     griddep_wait();                                       // (the bulk kernel's findings from here on)
     const SegPlan p = a.s.plan[seg];                      // (resume_chunk is the segment's first chunk: k_prime2)
+    const uint2 fw = lane < 9u ? a.s.usage_fields[(size_t)seg * 9u + lane] : make_uint2(0u, 0xFFFFFFFFu);   // (requested with the plan, used when has_cand)
     const StepIO io = make_io(a, slot, &st);
     uint32_t emit_begin = p.emit_chunk_begin;
     const bool speculated = p.kept_chunk != 0xFFFFFFFFu;
@@ -1390,26 +1384,30 @@ k_commit2(StepArgs a) {
         const uint32_t ups = (uint32_t)(p.last_usage >> 32) - 1u, ulen = (uint32_t)p.last_usage;
         const bool staged = p.last_usage && ulen <= LGW_PENDING_CAP && (uint64_t)ups + ulen <= a.n_bytes;
         const bool has_cand = staged && p.cand_ps == ups + 1u;
-        uint2 fld = make_uint2(0u, 0xFFFFFFFFu), gf = make_uint2(0u, 0u);
-        if (has_cand) { const uint2* uf = a.s.usage_fields + (size_t)seg * 9u; if (lane < 8u) fld = uf[lane]; gf = uf[8]; }
+        const uint2 fld = has_cand && lane < 8u ? fw : make_uint2(0u, 0xFFFFFFFFu);
+        const uint32_t g_slot = __shfl_sync(R2_FULL, fw.x, 8), g_flags = __shfl_sync(R2_FULL, fw.y, 8);
+        if (has_cand) {                                   // the template event's own UsageRaw, requested together with the text
+            const uint32_t* src = reinterpret_cast<const uint32_t*>(&a.s.tpl_cache2->raw[g_slot]);
+            for (uint32_t k = lane; k < sizeof(UsageRaw) / 4; k += 32) reinterpret_cast<uint32_t*>(stage_raw)[k] = src[k];
+        }
         // staged as whole 16-byte vectors around the text (the step's buffer is 16-byte aligned: the bulk kernel's TMA needs that too);
         // a vector that would reach beyond the step's bytes is read byte by byte
         const uint32_t ab = ups & ~15u, skew = ups - ab;
         const bool d_aligned = (reinterpret_cast<uintptr_t>(d) & 15u) == 0u;
-        const uint8_t* const utext = stage[warp] + skew;
+        const uint8_t* const utext = stage + skew;
         if (staged) {
             const uint32_t nvec = (skew + ulen + 15u) >> 4;
             for (uint32_t k = lane; k < nvec; k += 32) {
                 const uint32_t o = ab + (k << 4);
-                if (o + 16u <= a.n_bytes && d_aligned) *reinterpret_cast<uint4*>(stage[warp] + (k << 4)) = commit_ld16(d + o);
-                else for (uint32_t j = 0; j < 16u && o + j < a.n_bytes; ++j) stage[warp][(k << 4) + j] = __ldg(d + o + j);
+                if (o + 16u <= a.n_bytes && d_aligned) *reinterpret_cast<uint4*>(stage + (k << 4)) = commit_ld16(d + o);
+                else for (uint32_t j = 0; j < 16u && o + j < a.n_bytes; ++j) stage[(k << 4) + j] = __ldg(d + o + j);
             }
         }
         bool sequential = p.irregular || p.n_usage_b > 1 || any_empty;   // several usage candidates: let the exact path count them
         if (st.phase == PH_PRIMING && !(speculated && p.prime_ok)) sequential = true;
         if (!sequential && p.last_usage && !staged) sequential = true;
         if (!sequential && p.tail_start == 0xFFFFFFFFu) sequential = true;                        // (nobody reached the end of the text)
-        if (lane == 0) atomicAdd(a.s.counters + (sequential ? 0 : 1), 1u);
+        if (lane == 0) atomicAdd(&counts[sequential ? 0 : 1], 1u);
         if (sequential) {
             if (lane == 0) emit_begin = commit_sequential(io, a.data, a.chunk_off, p.resume_chunk, c1, (st.phase == PH_COMMITTED) ? p.resume_chunk : c1);
         } else {
@@ -1430,14 +1428,13 @@ k_commit2(StepArgs a) {
                 __syncwarp();
                 if (has_cand) {
                     // the bulk kernel matched it against a usage template and noted where the eight fields sit: read them out
-                    commit_usage_fields(utext, ups, ulen, gf.y, &a.s.tpl_cache2->raw[gf.x], &stage_raw[warp], io.rec, lane, fld.x, fld.y);
-                    __syncwarp();
+                    const uint32_t exotic = commit_usage_fields(utext, ups, ulen, g_flags, stage_raw, io.rec, lane, fld.x, fld.y);
                     st.flags |= SF_REC_VALID; ++st.n_usage_b;
-                    if (io.rec->exotic) { ++st.n_exotic; st.flags |= SF_EXOTIC_SEEN; }
-                    if (lane == 0) atomicAdd(a.s.counters + 2, 1u);
+                    if (exotic) { ++st.n_exotic; st.flags |= SF_EXOTIC_SEEN; }
+                    if (lane == 0) atomicAdd(&counts[2], 1u);
                 } else {
                     // no usage template: read the values out of the staged text with the full machine now
-                    if (lane == 0) { commit_usage_event(io, utext, ulen); atomicAdd(a.s.counters + 3, 1u); }
+                    if (lane == 0) { commit_usage_event(io, utext, ulen); atomicAdd(&counts[3], 1u); }
                 }
             }
             // new carry = text after the last separator (both loops: SF_SYNCED)
@@ -1453,6 +1450,28 @@ k_commit2(StepArgs a) {
         fill_seg_result(st, emit_begin, c1, res);
         a.seg_out[seg] = res;
     }
+}
+
+R2_GLOBAL void
+#if !R2_HOST_EMU
+__launch_bounds__(R2_CWARPS * 32, R2_CBLOCKS)      // (the full machine behind commit_usage_event / commit_sequential spills instead of costing every warp 142 registers)
+#endif
+k_commit2(StepArgs a) {
+#if !R2_HOST_EMU
+    __shared__ __align__(16) uint8_t stage[R2_CWARPS][LGW_PENDING_STRIDE];           // the winning usage event's text
+    __shared__ __align__(16) UsageRaw stage_raw[R2_CWARPS];                           // the record being assembled from it
+    __shared__ uint32_t counts[4];                                                  // the block's share of StepScratch::counters, added to them once
+#else
+    alignas(16) static uint8_t stage[R2_CWARPS][LGW_PENDING_STRIDE];
+    static UsageRaw stage_raw[R2_CWARPS];
+    static uint32_t counts[4];
+#endif
+    const uint32_t seg = (R2_BID * R2_NTHR + R2_TID) >> 5, lane = R2_TID & 31u, warp = (R2_TID >> 5) % R2_CWARPS;
+    if (R2_TID < 4) counts[R2_TID] = 0;
+    __syncthreads();
+    if (seg < a.n_segs) commit_one(a, seg, lane, stage[warp], &stage_raw[warp], counts);
+    __syncthreads();
+    if (R2_TID < 4 && counts[R2_TID]) atomicAdd(a.s.counters + R2_TID, counts[R2_TID]);
 }
 
 #if !R2_HOST_EMU

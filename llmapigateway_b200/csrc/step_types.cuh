@@ -52,6 +52,7 @@ struct StepArgs {
     const uint32_t* seg_chunk; const uint32_t* seg_slot; uint32_t n_segs;
     uint8_t* out; SegResult* seg_out;
     RowEvent* rowq; uint32_t* rowq_count; uint32_t rowq_cap;
+    uint32_t reset_rows;                       // 1: k_prime2 empties the row queue (the first launch of a step)
     StepScratch s;
 };
 
