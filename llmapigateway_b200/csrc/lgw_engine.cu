@@ -370,15 +370,9 @@ extern "C" int lgw_sse_step(lgw_engine* e, const uint8_t* bytes, uint64_t n_byte
     uint32_t n_slices = n_bytes >= (8u << 20) && n_segs >= 16 ? 8u : 1u;
     if (direct_in && direct_out) n_slices = 1;
     if (const char* sl = getenv("LGW_SLICES")) { int v = atoi(sl); if (v >= 1 && v <= 14) n_slices = (uint32_t)v; }
-    if (e->mode == 1 || n_segs < n_slices) n_slices = 1;
-    uint32_t cut[18]; cut[0] = 0;
-    for (uint32_t j = 1; j < n_slices; ++j) {           // segment index whose start byte is closest below j/n of the bytes
-        const uint64_t want = n_bytes * j / n_slices;
-        uint32_t lo = cut[j - 1], hi = n_segs;
-        while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if ((uint64_t)chunk_off[seg_chunk[mid]] < want) lo = mid + 1; else hi = mid; }
-        cut[j] = lo;
-    }
-    cut[n_slices] = n_segs;
+    if (e->mode == 1) n_slices = 1;
+    uint32_t cut[18];
+    n_slices = step_slice_cuts(n_bytes, chunk_off, seg_chunk, n_segs, n_slices, cut);
     CK(e, cudaMemsetAsync(e->d_rowq_count, 0, 4, e->stream));
     const bool piped = n_slices > 1;
     cudaStream_t sin = piped ? e->s_in : e->stream, sout = piped ? e->s_out : e->stream;

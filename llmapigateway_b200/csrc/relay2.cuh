@@ -1248,11 +1248,14 @@ R2_GLOBAL void k_prime2(StepArgs a) {
         } else if (c < c1) p.irregular = 1;                                    // an event is open from an earlier step
     }
     a.s.plan[seg] = p;
-    // the byte tiles whose first byte lies in this segment: where the bulk kernel's warps start looking
+    // the byte tiles whose first byte lies in this segment: where the bulk kernel's warps start looking.  Tile 0 starts at
+    // tile_base & ~15, before the launch's first byte when a slice starts unaligned: the first segment WITH bytes claims it
+    // (b0 == tile_base), even when segments without bytes come before it -- else nobody writes tile_seg[0] and warp 0 starts
+    // from whatever an earlier launch left there, which may skip the text it owns
     const uint32_t base0 = a.tile_base & ~15u;
     const uint32_t b0 = a.chunk_off[c0], b1 = p.seg_end;
     if (b1 > b0) {
-        uint32_t t_lo = seg == 0 ? 0u : (b0 - base0 + R2_TILE - 1) / R2_TILE;        // (tile 0 starts at the launch's first byte)
+        uint32_t t_lo = b0 == a.tile_base ? 0u : (b0 - base0 + R2_TILE - 1) / R2_TILE;
         const uint32_t t_hi = (b1 - 1 - base0) / R2_TILE;
         for (uint32_t t = t_lo; t <= t_hi; ++t) a.s.tile_seg[t] = seg;
     }

@@ -38,7 +38,8 @@ struct StepScratch {
     TemplateCache2* tpl_cache2;  // event templates, persistent across steps
     uint2* usage_fields;       // [max_streams][9] a template-following usage event of this step: (start, length | escapes << 31) of its eight
                                //   usage fields as the match located them, [8].x = the template's slot in the engine-wide cache
-    uint32_t* tile_seg;        // [max tiles + 1] segment that holds the first byte of each 4 KiB tile of the launch
+    uint32_t* tile_seg;        // [max tiles + 1] segment that holds the first byte of each 3 KiB tile of the launch (tile 0: the
+                               //   launch's first segment with bytes, since its first byte may lie before the launch)
     uint32_t* counters;        // diagnostics since engine creation: [0] segments redone sequentially, [1] segments folded from the bulk
                                //   kernel's findings, [2] usage records read from template spans, [3] usage events stashed
 };
@@ -47,14 +48,33 @@ struct StepArgs {
     DeviceTables t;
     const uint8_t* data; uint32_t n_bytes;     // n_bytes = end of the valid bytes (a slice of a pipelined step ends earlier)
     const uint32_t* chunk_off; uint32_t n_chunks;
-    uint32_t tile_base;                        // byte offset of tile 0 (multiple of LGW_TILE_BYTES)
-    uint32_t chunk_lo, chunk_hi;               // chunks of this launch: [chunk_lo, chunk_hi)
+    uint32_t tile_base;                        // first byte of the launch (a slice's start: any offset); tile 0 starts at tile_base & ~15
+    uint32_t chunk_lo, chunk_hi;               // chunks of this launch: [chunk_lo, chunk_hi).  No kernel reads them: they describe the
+                                               //   launch to a debugger, and the host build of the kernels (tests/support) fills them
     const uint32_t* seg_chunk; const uint32_t* seg_slot; uint32_t n_segs;
     uint8_t* out; SegResult* seg_out;
     RowEvent* rowq; uint32_t* rowq_count; uint32_t rowq_cap;
     uint32_t reset_rows;                       // 1: k_prime2 empties the row queue (the first launch of a step)
     StepScratch s;
 };
+
+// The slices of a host-buffer step (lgw_sse_step): slice j is segments [cut[j], cut[j + 1]), cut[j] = the first segment whose
+// start byte is >= n_bytes * j / n_slices.  So a slice may be empty, and a cut lands on a segment without bytes when one starts
+// there.  Fewer segments than slices: one slice.  Returns the number of slices; cut has room for n_slices + 1 entries.
+// (The host build of the kernels in tests/support slices with this same function.)
+static inline uint32_t step_slice_cuts(uint64_t n_bytes, const uint32_t* chunk_off, const uint32_t* seg_chunk, uint32_t n_segs,
+                                       uint32_t n_slices, uint32_t* cut) {
+    if (n_segs < n_slices) n_slices = 1;
+    cut[0] = 0;
+    for (uint32_t j = 1; j < n_slices; ++j) {
+        const uint64_t want = n_bytes * j / n_slices;
+        uint32_t lo = cut[j - 1], hi = n_segs;
+        while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if ((uint64_t)chunk_off[seg_chunk[mid]] < want) lo = mid + 1; else hi = mid; }
+        cut[j] = lo;
+    }
+    cut[n_slices] = n_segs;
+    return n_slices;
+}
 
 LGW_HD StepIO make_io(const StepArgs& a, uint32_t slot, StreamHdr* local_hdr) {
     StepIO io;
