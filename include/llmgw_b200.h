@@ -241,6 +241,16 @@ int lgw_rollup_buckets_of(const int64_t* ts_us, uint64_t n, int period, int64_t*
 int lgw_rollup_set_path(lgw_engine* e, int force_global);
 int lgw_rollup_last_ms(lgw_engine* e, float ms[2]);
 
+/* /v1/api/usage-records (tokens_usage_db.py:69-117): the record indices at ranks [first, first + count) of the order
+ * (ts_us DESC, index ASC) over n device-resident timestamps; idx_out is host memory.  n >= 2^32 or first + count > n: LGW_ERR_ARG
+ * (so is a d_ts_us that is not 16-byte aligned; cudaMalloc memory is).  Equal timestamps list in index (insertion) order.
+ * Device work: a radix select of the keys at both ends of the page (12 passes of 8-bit digits over the timestamp and the
+ * index; the passes read only the candidates once they are at most n/16), one ordered compaction of the page, and a sort of
+ * it: in one block up to 8192 records, a stable LSD radix sort above (csrc/listing.cuh).  count == 0 launches nothing. */
+int lgw_usage_latest(lgw_engine* e, const int64_t* d_ts_us, uint64_t n, uint64_t first, uint64_t count, uint64_t* idx_out);
+/* device time of the last lgw_usage_latest, milliseconds (0 after a call with count == 0) */
+int lgw_usage_latest_last_ms(lgw_engine* e, float* ms);
+
 /* ---- request-body rewrite: SURVEY 8 rows a1, a3, a4 --------------------------------------------------
  * Replaces, for a batch of client requests, chat.py:31-45 (parse: lgw_bodies_scan) and, per upstream
  * attempt, chat.py:112-119,:135-139,:150,:164-168 (deepcopy + key assignments) followed by the encoder

@@ -10,6 +10,7 @@
 #include "stream_machine.cuh"
 #include "sse_kernels.cuh"
 #include "rollup.cuh"
+#include "listing.cuh"
 #include "body_kernels.cuh"
 #include "doc_kernels.cuh"
 #include "transcript.cuh"
@@ -48,6 +49,9 @@ struct lgw_engine {
     RollupRow* d_rows = nullptr; uint64_t d_rows_cap = 0; unsigned long long* d_nrows = nullptr;
     uint8_t* d_partial = nullptr; size_t d_partial_cap = 0; uint32_t* d_tiles = nullptr; uint32_t d_tiles_cap = 0;
     bool rollup_attr_set = false, rollup_force_global = false;
+    // record listing (listing.cuh): one grow-only scratch buffer, events created on first use
+    uint8_t* l_buf = nullptr; size_t l_cap = 0;
+    cudaEvent_t lev[2]{}; float lms = 0; bool list_attr_set = false;
     uint8_t* d_details = nullptr; size_t d_details_cap = 0;      // staging of lgw_streams_details
     bool last_direct = false;       // the last host-buffer step ran in direct mode (kernel-driven PCIe traffic)
     float ms[5]{0, 0, 0, 0, 0};     // prime, relay, commit, usage extract, whole host-buffer step
@@ -147,6 +151,8 @@ extern "C" int lgw_engine_destroy(lgw_engine* e) {
     for (auto& ev : e->ev) if (ev) cudaEventDestroy(ev);
     for (auto& ev : e->rev) if (ev) cudaEventDestroy(ev);
     cudaFree(e->d_rows); cudaFree(e->d_nrows); cudaFree(e->d_partial); cudaFree(e->d_tiles); cudaFree(e->d_details);
+    cudaFree(e->l_buf);
+    for (auto& ev : e->lev) if (ev) cudaEventDestroy(ev);
     cudaFree(e->d_plans); cudaFree(e->d_ops); cudaFree(e->d_blob);
     cudaFree(e->b_in); cudaFree(e->b_slots); cudaFree(e->b_out); cudaFree(e->b_models); cudaFree(e->b_off); cudaFree(e->b_out_off);
     cudaFree(e->b_plan_idx); cudaFree(e->b_results); cudaFree(e->b_scans); cudaFree(e->b_redo);
@@ -588,6 +594,85 @@ extern "C" int lgw_rollup_last_ms(lgw_engine* e, float ms[2]) {
     if (cudaEventElapsedTime(&t, e->rev[0], e->rev[1]) == cudaSuccess) e->rms[0] = t;
     if (cudaEventElapsedTime(&t, e->rev[2], e->rev[3]) == cudaSuccess) e->rms[1] = t;
     ms[0] = e->rms[0]; ms[1] = e->rms[1];
+    return LGW_OK;
+}
+
+// ---- record listing (SURVEY.md 8(f) rank 2; tokens_usage_db.py:69-117) --------------------------------------------------------
+extern "C" int lgw_usage_latest(lgw_engine* e, const int64_t* d_ts_us, uint64_t n, uint64_t first, uint64_t count, uint64_t* idx_out) {
+    if (!e || n >= (1ull << 32) || count > n || first > n - count) return LGW_ERR_ARG;
+    if (count && (!d_ts_us || !idx_out || ((uintptr_t)d_ts_us & 15))) return LGW_ERR_ARG;
+    e->lms = 0;
+    if (!count) return LGW_OK;
+    CK(e, cudaSetDevice(e->device));
+    const uint32_t N = (uint32_t)n, M = (uint32_t)count, cap = N / LGW_LIST_CAND_DIV;
+    const uint32_t ctiles = (N + LGW_LIST_CTILE - 1) / LGW_LIST_CTILE, stiles = (M + LGW_LIST_STILE - 1) / LGW_LIST_STILE;
+    const size_t scan_n = ctiles > 256ull * stiles ? ctiles : 256ull * stiles;
+    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
+    const size_t o_cand = al(sizeof(ListSel)), o_keys = o_cand + al((size_t)(cap ? cap : 1) * sizeof(ListPair));
+    const size_t o_idx = o_keys + al((size_t)M * 16), o_out = o_idx + al((size_t)M * 8), o_scan = o_out + al((size_t)M * 8);
+    const size_t need = o_scan + al((scan_n + 257) * 4);
+    if (need > e->l_cap) {
+        cudaFree(e->l_buf); e->l_buf = nullptr; e->l_cap = 0;
+        CK(e, cudaMalloc((void**)&e->l_buf, need));
+        e->l_cap = need;
+    }
+    if (!e->lev[0]) for (auto& ev : e->lev) CK(e, cudaEventCreate(&ev));
+    if (!e->list_attr_set) {
+        CK(e, cudaFuncSetAttribute(k_list_sort_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(LGW_LIST_SMEM_SORT * 12)));
+        e->list_attr_set = true;
+    }
+    ListSel* sel = (ListSel*)e->l_buf;
+    ListPair* cand = (ListPair*)(e->l_buf + o_cand);
+    uint64_t* keys[2] = {(uint64_t*)(e->l_buf + o_keys), (uint64_t*)(e->l_buf + o_keys) + M};
+    uint32_t* idx[2] = {(uint32_t*)(e->l_buf + o_idx), (uint32_t*)(e->l_buf + o_idx) + M};
+    uint64_t* out = (uint64_t*)(e->l_buf + o_out);
+    uint32_t* scan = (uint32_t*)(e->l_buf + o_scan);
+    uint32_t* totals = scan + scan_n;                   // [256] column totals of the LSD scans
+    uint32_t* selected = totals + 256;                  // records between the two boundaries (== count)
+    const uint32_t pairs = (uint32_t)(((uint64_t)N + 1) / 2);
+    const uint32_t want = (pairs + 255) / 256, grid = want < (uint32_t)e->sm_count * 8 ? want : (uint32_t)e->sm_count * 8;
+    CK(e, cudaEventRecord(e->lev[0], e->stream));
+    k_list_init<<<1, 256, 0, e->stream>>>(sel, first, first + count - 1);
+    for (int d = 0; d < LGW_LIST_DIGITS; ++d) {
+        k_list_hist<<<grid, 256, 0, e->stream>>>(d_ts_us, N, cand, sel, d);
+        k_list_pick<<<1, 256, 0, e->stream>>>(sel, d, cap);
+        if (d + 1 < LGW_LIST_DIGITS) k_list_cand<<<grid, 256, 0, e->stream>>>(d_ts_us, N, cand, sel, d + 1);
+    }
+    k_list_tile_count<<<ctiles, 1024, 0, e->stream>>>(d_ts_us, N, sel, scan);
+    k_list_scan<<<1, 1024, 0, e->stream>>>(scan, ctiles, selected);
+    k_list_tile_write<<<ctiles, 1024, 0, e->stream>>>(d_ts_us, N, sel, scan, keys[0], idx[0]);
+    e->launches += 1 + 3 * LGW_LIST_DIGITS - 1 + 3;
+    if (M <= LGW_LIST_SMEM_SORT) {
+        uint32_t p = 1;
+        while (p < M) p <<= 1;
+        k_list_sort_small<<<1, 1024, (size_t)p * 12, e->stream>>>(keys[0], idx[0], M, out);
+        ++e->launches;
+    } else {
+        int cur = 0;
+        for (int shift = 0; shift < 64; shift += 8, cur ^= 1) {
+            k_lsd_hist<<<stiles, 256, 0, e->stream>>>(keys[cur], M, shift, scan, stiles);
+            k_list_scan<<<256, 1024, 0, e->stream>>>(scan, stiles, totals);
+            k_lsd_scatter<<<stiles, 256, 0, e->stream>>>(keys[cur], idx[cur], M, shift, scan, totals, stiles, keys[cur ^ 1], idx[cur ^ 1]);
+        }
+        const uint32_t wg = (M + 255) / 256 < (uint32_t)e->sm_count * 8 ? (M + 255) / 256 : (uint32_t)e->sm_count * 8;
+        k_list_widen<<<wg, 256, 0, e->stream>>>(idx[cur], M, out);
+        e->launches += 8 * 3 + 1;
+    }
+    CK(e, cudaEventRecord(e->lev[1], e->stream));
+    CK(e, cudaGetLastError());
+    uint32_t got = 0;
+    CK(e, cudaMemcpyAsync(idx_out, out, (size_t)M * 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(&got, selected, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    float t = 0;
+    if (cudaEventElapsedTime(&t, e->lev[0], e->lev[1]) == cudaSuccess) e->lms = t;
+    if (got != M) { e->err = "usage listing: " + std::to_string(got) + " records between the boundary keys, expected " + std::to_string(M); return LGW_ERR_CUDA; }
+    return LGW_OK;
+}
+
+extern "C" int lgw_usage_latest_last_ms(lgw_engine* e, float* ms) {
+    if (!e || !ms) return LGW_ERR_ARG;
+    *ms = e->lms;
     return LGW_OK;
 }
 

@@ -3,6 +3,7 @@ llm_gateway_core/db/tokens_usage_db.py (TokensUsageDB) for rows a10/a11 of SURVE
 
   UsageTable.insert_usage(d)         <- TokensUsageDB.insert_usage          (:119-162)
   UsageTable.get_aggregated_usage()  <- TokensUsageDB.get_aggregated_usage  (:222-304)  [GPU kernel]
+  UsageTable.get_latest_usage_records() <- TokensUsageDB.get_latest_usage_records (:69-117) [GPU kernel: page selection]
   stats_window(period, now)          <- llm_gateway_core/api/v1/stats.py:46-55
 
 Records live as SoA columns (40 B/record) in HBM; `model` is dictionary-encoded at ingest and
@@ -23,6 +24,8 @@ from . import _native
 PERIODS = {"hour": 0, "day": 1, "week": 2, "month": 3}
 _EPOCH = datetime(1970, 1, 1)
 ROLLUP_CELLS = 10
+# the record listing merges up to this many rows inserted since the last upload on the host; more, and it uploads the table again
+LISTING_PENDING_MAX = 65536
 
 ROW_DTYPE = np.dtype([("bucket", "<i8"), ("model_rank", "<i4"), ("inexact", "<u4"), ("prompt_tokens", "<i8"),
                       ("completion_tokens", "<i8"), ("total_tokens", "<i8"), ("reasoning_tokens", "<i8"),
@@ -90,6 +93,7 @@ class UsageTable:
         self._models: list[str | None] = []      # per record, until encoded
         self._providers: list[str | None] = []   # per record (listing only; the rollup does not group by provider)
         self._dev = None                          # (n, {col: device ptr}, names)
+        self._dev_n = None                        # records [0, _dev_n) of the host copy are on the device (inserts only append)
         self._pending_rows: list[tuple] = []
         self.rejected = 0                         # records insert_usage refused (see there)
 
@@ -139,6 +143,7 @@ class UsageTable:
         self._providers = [None] * len(self._models)
         self._pending_rows = []
         self._dev = None
+        self._dev_n = None
 
     def _materialise(self):
         if self._pending_rows:
@@ -162,6 +167,7 @@ class UsageTable:
         """Give the device copy of the columns back (an insert makes it stale; without this every re-upload would leak the last one)."""
         ptrs, self._dev_ptrs = getattr(self, "_dev_ptrs", None), None
         self._dev = None
+        self._dev_n = None
         if ptrs and getattr(self.eng, "_h", None):
             for p in ptrs.values():
                 self._lib.lgw_device_free(self.eng._h, p)
@@ -184,6 +190,7 @@ class UsageTable:
             self.eng._ck(self._lib.lgw_device_upload(self.eng._h, p, a.ctypes.data_as(C.c_void_p), a.nbytes), "device_upload")
             ptrs[c] = p
         self._dev = (n, ptrs)
+        self._dev_n = n
 
     def __len__(self):
         return int(self._host["ts_us"].size) + len(self._pending_rows)
@@ -318,29 +325,80 @@ class UsageTable:
         return len(self)
 
     def get_latest_usage_records(self, limit: int = 25, offset: int = 0) -> list[dict]:
-        """tokens_usage_db.py:69-117: newest first (`ORDER BY timestamp DESC LIMIT ? OFFSET ?`), same keys.  Host
-        side: a page of 25 rows out of the host copy of the columns is not GPU work.  Records with equal
-        timestamps come in insertion order (SQLite leaves their order unspecified)."""
+        """tokens_usage_db.py:69-117: newest first (`ORDER BY timestamp DESC LIMIT ? OFFSET ?`), same keys.  Records with
+        equal timestamps come in insertion order (SQLite leaves their order unspecified).  With an engine the page is
+        selected on the device (_latest_on_device) from the uploaded timestamps, and rows inserted since the upload are
+        merged on the host; without one, from the host copy of the columns."""
+        if self.eng is not None:
+            return self._latest_records_device(limit, offset)
         self._materialise()
         h = self._host
         n = int(h["ts_us"].size)
         if limit < 0:
             limit = n                                           # SQLite: a negative LIMIT means no limit
         order = np.argsort(-h["ts_us"], kind="stable")[max(offset, 0):max(offset, 0) + limit]
-        out = []
-        for i in order:
-            i = int(i)
-            out.append({"id": i + 1, "timestamp": (_EPOCH + timedelta(microseconds=int(h["ts_us"][i]))).isoformat(),
-                        "prompt_tokens": int(h["prompt_tokens"][i]), "completion_tokens": int(h["completion_tokens"][i]),
-                        "total_tokens": int(h["total_tokens"][i]), "reasoning_tokens": int(h["reasoning_tokens"][i]),
-                        "cached_tokens": int(h["cached_tokens"][i]), "cost": _sql_value(float(h["cost"][i])),
-                        "model": self._models[i], "provider": self._providers[i]})
-        return out
+        return [self._record(int(i)) for i in order]
+
+    def _record(self, i: int) -> dict:
+        """record i as a listing row; i may be a row inserted since the host columns were last built"""
+        h = self._host
+        n_host = int(h["ts_us"].size)
+        if i < n_host:
+            ts, model, provider = int(h["ts_us"][i]), self._models[i], self._providers[i]
+            tok = [int(h[c][i]) for c in self.COLS[2:7]]
+            cost = float(h["cost"][i])
+        else:
+            ts, model, *tok, cost, provider = self._pending_rows[i - n_host]
+        return {"id": i + 1, "timestamp": (_EPOCH + timedelta(microseconds=int(ts))).isoformat(),
+                "prompt_tokens": int(tok[0]), "completion_tokens": int(tok[1]), "total_tokens": int(tok[2]),
+                "reasoning_tokens": int(tok[3]), "cached_tokens": int(tok[4]), "cost": _sql_value(float(cost)),
+                "model": model, "provider": provider}
+
+    def _latest_on_device(self, n: int, first: int, count: int) -> np.ndarray:
+        """indices of the uploaded records [0, n) at ranks [first, first + count) of (ts_us DESC, index ASC)"""
+        idx = np.empty(count, np.uint64)
+        self.eng._ck(self._lib.lgw_usage_latest(self.eng._h, self._dev_ptrs["ts_us"], n, first, count,
+                                                idx.ctypes.data_as(C.c_void_p)), "usage_latest")
+        return idx
+
+    def _latest_records_device(self, limit: int, offset: int) -> list[dict]:
+        total = len(self)
+        if limit < 0:
+            limit = total                                       # SQLite: a negative LIMIT means no limit
+        offset = max(offset, 0)
+        if limit == 0 or offset >= total:
+            return []
+        if self._dev_n is None or total - self._dev_n > LISTING_PENDING_MAX:
+            self._upload()                                      # (both cases have _dev None: a load, or inserts since the upload)
+        n_dev = self._dev_n
+        p = total - n_dev
+        if p == 0:
+            return [self._record(int(i)) for i in self._latest_on_device(n_dev, offset, min(limit, total - offset))]
+        # Rows n_dev .. total-1 are not on the device; all of them sort after the uploaded ones on equal timestamps.  A page
+        # row from the device has an uploaded rank in [offset - p, offset + limit): select those, merge with the pending rows.
+        lo = max(0, offset - p)
+        hi = min(n_dev, offset + limit)
+        dev_idx = self._latest_on_device(n_dev, lo, hi - lo).astype(np.int64) if hi > lo else np.zeros(0, np.int64)
+        h_ts = self._host["ts_us"]
+        pend_ts = np.concatenate([h_ts[n_dev:], np.array([r[0] for r in self._pending_rows], np.int64)])
+        idx = np.concatenate([dev_idx, np.arange(n_dev, total, dtype=np.int64)])
+        ts = np.concatenate([h_ts[dev_idx], pend_ts])
+        merged = idx[np.lexsort((idx, ~ts))]                   # (~ts: descending, without -ts's overflow at INT64_MIN)
+        # merged position j >= p holds global rank lo + j when lo > 0 (pending rows before uploaded rank lo rank below offset);
+        # every position holds global rank j when lo == 0
+        start = offset - lo
+        return [self._record(int(i)) for i in merged[start:start + limit]]
 
     def last_ms(self):
         ms = (C.c_float * 2)()
         self.eng._ck(self._lib.lgw_rollup_last_ms(self.eng._h, C.byref(ms)), "rollup_last_ms")
         return {"accum": ms[0], "emit": ms[1]}
+
+    def listing_last_ms(self) -> float:
+        """device time of the last page selected on the device (0 when the last listing needed none)"""
+        ms = C.c_float()
+        self.eng._ck(self._lib.lgw_usage_latest_last_ms(self.eng._h, C.byref(ms)), "usage_latest_last_ms")
+        return ms.value
 
 
 def synth_usage_columns(n: int, seed: int = 5, end: datetime = datetime(2026, 9, 21, 6, 57, 17, 47518), days: int = 400, n_models: int = 64):
