@@ -28,63 +28,153 @@ static_assert(sizeof(TextMark) == sizeof(lgw_text_mark), "lgw_text_mark layout")
 
 static thread_local std::string g_create_error;
 
+// Grow-only device staging.  reserve() keeps the buffer while it is large enough; otherwise it frees it and allocates
+// need + slack bytes (cudaFree synchronises the device, so callers whose sizes creep upward pass a slack).  The contents do
+// not survive a growth.  Freed with the engine that holds it.
+struct DevBuf {
+    void* p = nullptr; size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
+    cudaError_t reserve(size_t need, size_t slack = 0) {
+        if (need <= cap) return cudaSuccess;
+        if (p) cudaFree(p);
+        p = nullptr; cap = 0;
+        const cudaError_t r = cudaMalloc(&p, need + slack);
+        if (r == cudaSuccess) cap = need + slack;
+        return r;
+    }
+    template <class T> T* as() const { return static_cast<T*>(p); }
+};
+
+// The arrays of one step as the kernels see them (device memory, or page-locked host memory in the direct modes).
+struct StepArrays {
+    const uint8_t* bytes; uint64_t n_bytes;
+    const uint32_t* chunk_off; uint32_t n_chunks;
+    const uint32_t *seg_chunk, *seg_slot; uint32_t n_segs;
+    uint8_t* out; SegResult* seg_out;
+};
+
+// One launch set's share of a step: segments [s0, s1), chunks [c0, c1), bytes [b0, b1).  All are absolute, so the slices of a
+// pipelined step share the device arrays.
+struct StepSlice {
+    uint32_t s0, s1, c0, c1, b0; uint64_t b1;
+    static StepSlice whole(uint32_t n_segs, uint32_t n_chunks, uint64_t n_bytes) { return {0, n_segs, 0, n_chunks, 0, n_bytes}; }
+};
+
 struct lgw_engine {
     int device = 0;
     lgw_limits lim{};
+    int sm_count = 132;
+    int mode = 0;                   // 0: fast path + general fix-up, 1: general path only
     cudaStream_t own_stream = nullptr, stream = nullptr;
     cudaStream_t s_in = nullptr, s_out = nullptr;       // copy streams of the pipelined host entry point
-    cudaEvent_t ev_in[16]{}, ev_k[16]{};
-    DeviceTables t{};               // persistent per-slot state
-    uint32_t* d_rowq_count = nullptr;
-    RowEvent* d_rowq = nullptr;
-    StepScratch scratch{};          // per-step scratch (sized by max_step_chunks / max_streams)
-    // staging for the host-pointer entry points
-    uint8_t *d_in = nullptr, *d_out = nullptr;
-    uint32_t *d_chunk_off = nullptr, *d_seg_chunk = nullptr, *d_seg_slot = nullptr;
-    SegResult* d_seg_out = nullptr;
-    uint32_t* d_slots = nullptr; int32_t* d_status = nullptr; StreamState* d_state_stage = nullptr;
-    cudaEvent_t ev[7]{};            // [0..4] bracket prime / relay / commit / usage extract; [5],[6] the host-buffer step
-    cudaEvent_t rev[4]{};
-    float rms[2]{0, 0};
-    RollupRow* d_rows = nullptr; uint64_t d_rows_cap = 0; unsigned long long* d_nrows = nullptr;
-    uint8_t* d_partial = nullptr; size_t d_partial_cap = 0; uint32_t* d_tiles = nullptr; uint32_t d_tiles_cap = 0;
-    bool rollup_attr_set = false, rollup_force_global = false;
-    // record listing (listing.cuh): one grow-only scratch buffer, events created on first use
-    uint8_t* l_buf = nullptr; size_t l_cap = 0;
-    cudaEvent_t lev[2]{}; float lms = 0; bool list_attr_set = false;
-    uint8_t* d_details = nullptr; size_t d_details_cap = 0;      // staging of lgw_streams_details
-    bool last_direct = false;       // the last host-buffer step ran in direct mode (kernel-driven PCIe traffic)
-    float ms[5]{0, 0, 0, 0, 0};     // prime, relay, commit, usage extract, whole host-buffer step
-    bool timed = false;
     uint64_t launches = 0;
-    // request-body rewrite (rows a1-a4): plan table + grow-only staging
-    BodyPlan* d_plans = nullptr; BodyOp* d_ops = nullptr; uint8_t* d_blob = nullptr; uint32_t n_plans = 0, n_ops = 0;
-    uint8_t *b_in = nullptr, *b_slots = nullptr, *b_out = nullptr, *b_models = nullptr;
-    uint64_t *b_off = nullptr, *b_out_off = nullptr; uint32_t* b_plan_idx = nullptr; BodyResult* b_results = nullptr; BodyScan* b_scans = nullptr;
-    uint64_t b_in_cap = 0, b_slots_cap = 0, b_out_cap = 0, b_n_cap = 0, b_models_cap = 0, b_redo_cap = 0;
-    uint32_t* b_redo = nullptr;
-    int body_mode = 0;              // 0: data-parallel path + exact machine for the rest, 1: exact machine only (tests)
-    cudaEvent_t bev[4]{};
-    float bms[3]{0, 0, 0};
-    bool per_kernel_timing = false; // true: events between the step's kernels (lgw_last_step_kernel_ms); false: programmatic dependent launches
-    bool kernel_times_valid = false;
-    int mode = 0;                   // 0: fast path + general fix-up, 1: general path only
-    int sm_count = 132;
-    // transcript tap (transcript.cuh; off until lgw_transcripts_enable)
-    bool text_on = false, text_pending = false, text_ready = false;
-    TextTap* d_tap = nullptr; uint8_t* d_tcarry = nullptr; uint8_t* d_tsparse = nullptr; uint8_t* d_ttext = nullptr;
-    uint32_t *d_piece_len = nullptr, *d_tseg_len = nullptr, *d_tseg_flags = nullptr, *d_markq_count = nullptr;
-    unsigned long long* d_tseg_off = nullptr; TextMark* d_markq = nullptr;
-    uint64_t text_total = 0; uint32_t text_marks = 0;
-    cudaEvent_t tev[2]{}; float tms = 0;
-    // the arrays of the last step (device-visible): what lgw_step_transcript_run works on
-    const uint8_t* last_bytes = nullptr; const uint32_t *last_chunk_off = nullptr, *last_seg_chunk = nullptr, *last_seg_slot = nullptr;
-    const SegResult* last_seg_out = nullptr; uint32_t last_n_chunks = 0, last_n_segs = 0; uint64_t last_n_bytes = 0;
     std::string err;
+    // What the engine owns on the device and how it goes away: fixed-size allocations (dev_alloc) and events (new_events)
+    // are recorded here and released by the destructor; grow-only staging is DevBuf members, which release themselves.
+    std::vector<void*> allocs;
+    std::vector<cudaEvent_t> events;
+    DeviceTables t{};               // persistent per-slot state
+    uint32_t* d_rowq_count = nullptr; RowEvent* d_rowq = nullptr;
+    StepScratch scratch{};          // per-step scratch (sized by max_step_chunks / max_streams)
+    uint32_t* d_slots = nullptr; int32_t* d_status = nullptr; StreamState* d_state_stage = nullptr;   // slot lists of open / state / close
+    DevBuf details;                 // staging of lgw_streams_details
+    struct Step {
+        uint8_t *d_in = nullptr, *d_out = nullptr;      // staging for the host-pointer entry point
+        uint32_t *d_chunk_off = nullptr, *d_seg_chunk = nullptr, *d_seg_slot = nullptr; SegResult* d_seg_out = nullptr;
+        cudaEvent_t ev_in[16]{}, ev_k[16]{};    // upload done / kernels done, per slice; [14] and [15] join the three streams at the step's ends
+        cudaEvent_t ev[7]{};            // [0..4] bracket prime / relay / commit / usage extract; [5],[6] the host-buffer step
+        cudaEvent_t tr[3][16]{};        // LGW_TRACE: upload / kernels / download done, per slice; created by the first traced step
+        float ms[5]{0, 0, 0, 0, 0};     // prime, relay, commit, usage extract, whole host-buffer step
+        bool timed = false, kernel_times_valid = false;
+        bool per_kernel_timing = false; // true: events between the step's kernels (lgw_last_step_kernel_ms); false: programmatic dependent launches
+        bool last_direct = false;       // the last host-buffer step ran in direct mode (kernel-driven PCIe traffic)
+        StepArrays last{};              // the arrays of the last step: what lgw_step_transcript_run works on
+    } step;
+    struct Rollup {
+        DevBuf rows, partial, tiles; unsigned long long* d_nrows = nullptr;
+        bool attr_set = false, force_global = false;
+        cudaEvent_t ev[4]{}; float ms[2]{0, 0};
+    } rollup;
+    struct Listing {                // record listing (listing.cuh): one scratch buffer, events created on first use
+        DevBuf buf; bool attr_set = false;
+        cudaEvent_t ev[2]{}; float ms = 0;
+    } listing;
+    struct Bodies {                 // request-body rewrite (rows a1-a4) and the document kernels, which share its input staging
+        DevBuf plans, ops, blob; uint32_t n_plans = 0, n_ops = 0;       // the rule tables of lgw_rules_load
+        DevBuf in, off, out_off, plan_idx, results, scans;      // per call: the packed bodies and five arrays indexed by body
+        DevBuf slots, out, models, redo;
+        DevBuf doc_out, doc_text;   // results of lgw_documents_usage / lgw_documents_error_detail
+        int mode = 0;               // 0: data-parallel path + exact machine for the rest, 1: exact machine only (tests)
+        cudaEvent_t ev[4]{}; float ms[3]{0, 0, 0};
+    } bodies;
+    struct Text {                   // transcript tap (transcript.cuh; off until lgw_transcripts_enable)
+        bool on = false, pending = false, ready = false;
+        TextTap* tap = nullptr; uint8_t *carry = nullptr, *sparse = nullptr, *text = nullptr;
+        uint32_t *piece_len = nullptr, *seg_len = nullptr, *seg_flags = nullptr, *markq_count = nullptr;
+        unsigned long long* seg_off = nullptr; TextMark* markq = nullptr;
+        uint64_t total = 0; uint32_t marks = 0;
+        cudaEvent_t ev[2]{}; float ms = 0;
+    } text;
+
+    ~lgw_engine() {                 // (the caller has made `device` current)
+        for (void* p : allocs) cudaFree(p);
+        for (cudaEvent_t ev : events) cudaEventDestroy(ev);
+        if (s_in) cudaStreamDestroy(s_in);
+        if (s_out) cudaStreamDestroy(s_out);
+        if (own_stream) cudaStreamDestroy(own_stream);
+    }
 };
 
 #define CK(e, call) do { cudaError_t _r = (call); if (_r != cudaSuccess) { \
     (e)->err = std::string(#call) + ": " + cudaGetErrorString(_r); return LGW_ERR_CUDA; } } while (0)
+// the same for a call that returns an LGW_* code (and has set e->err)
+#define TRY(call) do { const int _rc = (call); if (_rc != LGW_OK) return _rc; } while (0)
+
+// A fixed-size device allocation that lives as long as the engine.
+template <class T> static cudaError_t dev_alloc(lgw_engine* e, T*& p, size_t bytes) {
+    const cudaError_t r = cudaMalloc((void**)&p, bytes);
+    if (r == cudaSuccess) e->allocs.push_back(p);
+    return r;
+}
+
+// n events that live as long as the engine.
+static cudaError_t new_events(lgw_engine* e, cudaEvent_t* ev, int n, unsigned flags = cudaEventDefault) {
+    for (int i = 0; i < n; ++i) {
+        const cudaError_t r = cudaEventCreateWithFlags(&ev[i], flags);
+        if (r != cudaSuccess) return r;
+        e->events.push_back(ev[i]);
+    }
+    return cudaSuccess;
+}
+
+// ms = the time between two recorded events; kept as it was when they cannot be read (not recorded yet, or not complete).
+static void read_ms(cudaEvent_t from, cudaEvent_t to, float& ms) {
+    float t = 0;
+    if (cudaEventElapsedTime(&t, from, to) == cudaSuccess) ms = t;
+}
+
+// Blocks for n_items at per_block items a block, at most blocks_per_sm for each SM (the kernels stride over the rest).
+static unsigned grid_for(const lgw_engine* e, uint64_t n_items, uint32_t per_block, uint32_t blocks_per_sm) {
+    const uint64_t want = (n_items + per_block - 1) / per_block, most = (uint64_t)e->sm_count * blocks_per_sm;
+    return (unsigned)(want < most ? want : most);
+}
+
+static int check_slots(lgw_engine* e, const uint32_t* slots, uint32_t n) {
+    for (uint32_t i = 0; i < n; ++i) if (slots[i] >= e->lim.max_streams) { e->err = "slot out of range"; return LGW_ERR_ARG; }
+    return LGW_OK;
+}
+
+// A checked slot list into d_slots (which holds max_streams of them), on the engine stream.
+static int stage_slots(lgw_engine* e, const uint32_t* slots, uint32_t n) {
+    if (n > e->lim.max_streams) { e->err = "more slots than max_streams"; return LGW_ERR_CAPACITY; }
+    TRY(check_slots(e, slots, n));
+    CK(e, cudaSetDevice(e->device));
+    CK(e, cudaMemcpyAsync(e->d_slots, slots, n * 4, cudaMemcpyHostToDevice, e->stream));
+    return LGW_OK;
+}
 
 extern "C" int lgw_abi_version(void) { return LGW_ABI_VERSION; }
 
@@ -112,12 +202,13 @@ extern "C" int lgw_engine_create(int device, const lgw_limits* limits, lgw_engin
     e->stream = e->own_stream;
     if ((r = cudaStreamCreateWithFlags(&e->s_in, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", r);
     if ((r = cudaStreamCreateWithFlags(&e->s_out, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", r);
-    for (int i = 0; i < 16; ++i) { if ((r = cudaEventCreateWithFlags(&e->ev_in[i], cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", r); if ((r = cudaEventCreateWithFlags(&e->ev_k[i], cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", r); }
-    for (auto& ev : e->ev) if ((r = cudaEventCreate(&ev)) != cudaSuccess) return fail("cudaEventCreate", r);
-    for (auto& ev : e->rev) if ((r = cudaEventCreate(&ev)) != cudaSuccess) return fail("cudaEventCreate", r);
-    for (auto& ev : e->bev) if ((r = cudaEventCreate(&ev)) != cudaSuccess) return fail("cudaEventCreate", r);
+    if ((r = new_events(e, e->step.ev_in, 16, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", r);
+    if ((r = new_events(e, e->step.ev_k, 16, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", r);
+    if ((r = new_events(e, e->step.ev, 7)) != cudaSuccess) return fail("cudaEventCreate", r);
+    if ((r = new_events(e, e->rollup.ev, 4)) != cudaSuccess) return fail("cudaEventCreate", r);
+    if ((r = new_events(e, e->bodies.ev, 4)) != cudaSuccess) return fail("cudaEventCreate", r);
     const size_t S = e->lim.max_streams, C = e->lim.max_step_chunks, B = e->lim.max_step_bytes;
-#define ALLOC(ptr, bytes) if ((r = cudaMalloc((void**)&(ptr), (bytes))) != cudaSuccess) return fail("cudaMalloc " #ptr, r)
+#define ALLOC(ptr, bytes) if ((r = dev_alloc(e, ptr, (bytes))) != cudaSuccess) return fail("cudaMalloc " #ptr, r)
     ALLOC(e->t.state, S * sizeof(StreamState));
     ALLOC(e->t.carry_a, S * (size_t)e->lim.carry_cap);
     ALLOC(e->t.carry_b, S * (size_t)e->lim.carry_cap);
@@ -126,12 +217,12 @@ extern "C" int lgw_engine_create(int device, const lgw_limits* limits, lgw_engin
     e->t.carry_cap = e->lim.carry_cap; e->t.detail_cap = e->lim.detail_cap; e->t.max_streams = e->lim.max_streams;
     ALLOC(e->d_rowq, (size_t)(e->lim.rowq_cap + 1) * sizeof(RowEvent));
     ALLOC(e->d_rowq_count, 16);
-    ALLOC(e->d_in, B + 64); ALLOC(e->d_out, B + 64);
-    ALLOC(e->d_chunk_off, (C + 1) * 4); ALLOC(e->d_seg_chunk, (S + 1) * 4); ALLOC(e->d_seg_slot, S * 4);
-    ALLOC(e->d_seg_out, S * sizeof(SegResult));
+    ALLOC(e->step.d_in, B + 64); ALLOC(e->step.d_out, B + 64);
+    ALLOC(e->step.d_chunk_off, (C + 1) * 4); ALLOC(e->step.d_seg_chunk, (S + 1) * 4); ALLOC(e->step.d_seg_slot, S * 4);
+    ALLOC(e->step.d_seg_out, S * sizeof(SegResult));
     ALLOC(e->d_slots, S * 4); ALLOC(e->d_status, S * 4); ALLOC(e->d_state_stage, S * sizeof(StreamState));
-    if ((r = scratch_alloc(e->scratch, S, B, e->sm_count)) != cudaSuccess) return fail("scratch_alloc", r);
 #undef ALLOC
+    if ((r = scratch_alloc(e->scratch, S, B, [e](auto*& p, size_t bytes) { return dev_alloc(e, p, bytes); })) != cudaSuccess) return fail("scratch_alloc", r);
     if ((r = cudaMemset(e->t.state, 0, S * sizeof(StreamState))) != cudaSuccess) return fail("cudaMemset", r);
     if ((r = cudaMemset(e->d_rowq_count, 0, 16)) != cudaSuccess) return fail("cudaMemset", r);
     const char* m = getenv("LGW_FORCE_GENERAL");
@@ -143,27 +234,6 @@ extern "C" int lgw_engine_create(int device, const lgw_limits* limits, lgw_engin
 extern "C" int lgw_engine_destroy(lgw_engine* e) {
     if (!e) return LGW_OK;
     cudaSetDevice(e->device);
-    cudaFree(e->t.state); cudaFree(e->t.carry_a); cudaFree(e->t.carry_b); cudaFree(e->t.detail); cudaFree(e->t.pending);
-    cudaFree(e->d_rowq); cudaFree(e->d_rowq_count); cudaFree(e->d_in); cudaFree(e->d_out);
-    cudaFree(e->d_chunk_off); cudaFree(e->d_seg_chunk); cudaFree(e->d_seg_slot); cudaFree(e->d_seg_out);
-    cudaFree(e->d_slots); cudaFree(e->d_status); cudaFree(e->d_state_stage);
-    scratch_free(e->scratch);
-    for (auto& ev : e->ev) if (ev) cudaEventDestroy(ev);
-    for (auto& ev : e->rev) if (ev) cudaEventDestroy(ev);
-    cudaFree(e->d_rows); cudaFree(e->d_nrows); cudaFree(e->d_partial); cudaFree(e->d_tiles); cudaFree(e->d_details);
-    cudaFree(e->l_buf);
-    for (auto& ev : e->lev) if (ev) cudaEventDestroy(ev);
-    cudaFree(e->d_plans); cudaFree(e->d_ops); cudaFree(e->d_blob);
-    cudaFree(e->b_in); cudaFree(e->b_slots); cudaFree(e->b_out); cudaFree(e->b_models); cudaFree(e->b_off); cudaFree(e->b_out_off);
-    cudaFree(e->b_plan_idx); cudaFree(e->b_results); cudaFree(e->b_scans); cudaFree(e->b_redo);
-    for (auto& ev : e->bev) if (ev) cudaEventDestroy(ev);
-    cudaFree(e->d_tap); cudaFree(e->d_tcarry); cudaFree(e->d_tsparse); cudaFree(e->d_ttext); cudaFree(e->d_piece_len); cudaFree(e->d_tseg_len);
-    cudaFree(e->d_tseg_flags); cudaFree(e->d_markq_count); cudaFree(e->d_tseg_off); cudaFree(e->d_markq);
-    for (auto& ev : e->tev) if (ev) cudaEventDestroy(ev);
-    for (int i = 0; i < 16; ++i) { if (e->ev_in[i]) cudaEventDestroy(e->ev_in[i]); if (e->ev_k[i]) cudaEventDestroy(e->ev_k[i]); }
-    if (e->s_in) cudaStreamDestroy(e->s_in);
-    if (e->s_out) cudaStreamDestroy(e->s_out);
-    if (e->own_stream) cudaStreamDestroy(e->own_stream);
     delete e;
     return LGW_OK;
 }
@@ -176,27 +246,24 @@ extern "C" int lgw_engine_set_stream(lgw_engine* e, void* s) {
 
 extern "C" int lgw_engine_set_kernel_timing(lgw_engine* e, int on) {   // 1: CUDA events between the kernels of a step (they then run back to back, not overlapped)
     if (!e) return LGW_ERR_ARG;
-    e->per_kernel_timing = on != 0;
+    e->step.per_kernel_timing = on != 0;
     return LGW_OK;
 }
 
 extern "C" int lgw_engine_set_mode(lgw_engine* e, int mode) {     // 0 fast+fix-up, 1 general only (tests)
     if (!e) return LGW_ERR_ARG;
-    e->mode = mode; e->body_mode = mode;
+    e->mode = mode; e->bodies.mode = mode;
     return LGW_OK;
 }
 
 extern "C" int lgw_streams_open(lgw_engine* e, const uint32_t* slots, const int32_t* http_status, uint32_t n) {
     if (!e || !slots || !http_status) return LGW_ERR_ARG;
     if (n == 0) return LGW_OK;
-    if (n > e->lim.max_streams) { e->err = "more slots than max_streams"; return LGW_ERR_CAPACITY; }
-    for (uint32_t i = 0; i < n; ++i) if (slots[i] >= e->lim.max_streams) { e->err = "slot out of range"; return LGW_ERR_ARG; }
-    CK(e, cudaSetDevice(e->device));
-    CK(e, cudaMemcpyAsync(e->d_slots, slots, n * 4, cudaMemcpyHostToDevice, e->stream));
+    TRY(stage_slots(e, slots, n));
     CK(e, cudaMemcpyAsync(e->d_status, http_status, n * 4, cudaMemcpyHostToDevice, e->stream));
     k_streams_open<<<(n + 127) / 128, 128, 0, e->stream>>>(e->t, e->d_slots, e->d_status, n);
     ++e->launches;
-    if (e->text_on) { k_text_open<<<(n + 127) / 128, 128, 0, e->stream>>>(e->d_tap, e->d_slots, n); ++e->launches; }
+    if (e->text.on) { k_text_open<<<(n + 127) / 128, 128, 0, e->stream>>>(e->text.tap, e->d_slots, n); ++e->launches; }
     CK(e, cudaGetLastError());
     CK(e, cudaStreamSynchronize(e->stream));
     return LGW_OK;
@@ -205,10 +272,7 @@ extern "C" int lgw_streams_open(lgw_engine* e, const uint32_t* slots, const int3
 static int gather_states(lgw_engine* e, const uint32_t* slots, uint32_t n, lgw_stream_state* out, int free_after) {
     if (!e || !slots || !out) return LGW_ERR_ARG;
     if (n == 0) return LGW_OK;
-    if (n > e->lim.max_streams) { e->err = "more slots than max_streams"; return LGW_ERR_CAPACITY; }
-    for (uint32_t i = 0; i < n; ++i) if (slots[i] >= e->lim.max_streams) { e->err = "slot out of range"; return LGW_ERR_ARG; }
-    CK(e, cudaSetDevice(e->device));
-    CK(e, cudaMemcpyAsync(e->d_slots, slots, n * 4, cudaMemcpyHostToDevice, e->stream));
+    TRY(stage_slots(e, slots, n));
     k_streams_gather<<<(n + 127) / 128, 128, 0, e->stream>>>(e->t, e->d_slots, n, e->d_state_stage, free_after);
     ++e->launches;
     CK(e, cudaGetLastError());
@@ -252,16 +316,12 @@ __global__ void k_details_gather(DeviceTables t, const uint32_t* slots, uint32_t
 extern "C" int lgw_streams_details(lgw_engine* e, const uint32_t* slots, uint32_t n, uint8_t* buf, uint32_t stride, uint32_t* lens) {
     if (!e || (n && (!slots || !buf || !lens)) || stride == 0) return LGW_ERR_ARG;
     if (n == 0) return LGW_OK;
-    for (uint32_t i = 0; i < n; ++i) if (slots[i] >= e->lim.max_streams) return LGW_ERR_ARG;
+    TRY(check_slots(e, slots, n));
     CK(e, cudaSetDevice(e->device));
-    // grow-only staging owned by the engine (a stream-ordered allocation per call gave memory back to the OS at every synchronisation)
+    // staging owned by the engine (a stream-ordered allocation per call gave memory back to the OS at every synchronisation)
     const size_t need = (size_t)n * 8 + (size_t)n * stride;
-    if (need > e->d_details_cap) {
-        cudaFree(e->d_details); e->d_details = nullptr; e->d_details_cap = 0;
-        CK(e, cudaMalloc((void**)&e->d_details, need + need / 2));
-        e->d_details_cap = need + need / 2;
-    }
-    uint32_t* d_slots = (uint32_t*)e->d_details; uint32_t* d_lens = d_slots + n; uint8_t* d_out = e->d_details + (size_t)n * 8;
+    CK(e, e->details.reserve(need, need / 2));
+    uint32_t* d_slots = e->details.as<uint32_t>(); uint32_t* d_lens = d_slots + n; uint8_t* d_out = e->details.as<uint8_t>() + (size_t)n * 8;
     CK(e, cudaMemcpyAsync(d_slots, slots, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
     lgw::k_details_gather<<<(n * 32 + 255) / 256, 256, 0, e->stream>>>(e->t, d_slots, n, d_out, stride, d_lens);
     ++e->launches;
@@ -272,33 +332,37 @@ extern "C" int lgw_streams_details(lgw_engine* e, const uint32_t* slots, uint32_
 }
 
 // ---- the step ------------------------------------------------------------------------------------
-// One launch set over segments [s0, s1) of a step (the whole step when s0 = 0, s1 = n_segs).  All
-// offsets and chunk indices stay absolute, so slices of a pipelined step share the device arrays.
-static int step_device(lgw_engine* e, const uint8_t* d_bytes, uint64_t n_bytes, const uint32_t* d_chunk_off, uint32_t n_chunks,
-                       const uint32_t* d_seg_chunk, const uint32_t* d_seg_slot, uint32_t n_segs,
-                       uint8_t* d_out, SegResult* d_seg_out,
-                       uint32_t s0 = 0, uint32_t s1 = 0xFFFFFFFFu, uint32_t c0 = 0, uint32_t c1 = 0xFFFFFFFFu,
-                       uint32_t b0 = 0, uint64_t b1 = ~0ull, bool reset_rows = true) {
+static int check_step_limits(lgw_engine* e, uint32_t n_segs, uint32_t n_chunks, uint64_t n_bytes) {
     if (n_segs > e->lim.max_streams || n_chunks > e->lim.max_step_chunks || n_bytes > e->lim.max_step_bytes) {
         e->err = "step exceeds the limits given to lgw_engine_create"; return LGW_ERR_CAPACITY;
     }
     if (n_bytes >= 0xFFFF0000ull) { e->err = "step larger than 4 GiB - 64 KiB"; return LGW_ERR_CAPACITY; }
-    if (s1 == 0xFFFFFFFFu) { s1 = n_segs; c1 = n_chunks; b1 = n_bytes; }
+    return LGW_OK;
+}
+
+// The step the transcript pass will tap, once.
+static void remember_step(lgw_engine* e, const StepArrays& s) {
+    e->step.last = s;
+    e->text.pending = e->text.on; e->text.ready = false;
+}
+
+// One launch set over a slice of a step whose limits have been checked.
+static int step_device(lgw_engine* e, const StepArrays& s, const StepSlice& sl, bool reset_rows) {
     StepArgs a{};
-    a.t = e->t; a.data = d_bytes; a.n_bytes = (uint32_t)b1; a.chunk_off = d_chunk_off; a.n_chunks = n_chunks;
-    a.tile_base = b0; a.chunk_lo = c0; a.chunk_hi = c1;
-    a.seg_chunk = d_seg_chunk + s0; a.seg_slot = d_seg_slot + s0; a.n_segs = s1 - s0; a.out = d_out; a.seg_out = d_seg_out + s0;
+    a.t = e->t; a.data = s.bytes; a.n_bytes = (uint32_t)sl.b1; a.chunk_off = s.chunk_off; a.n_chunks = s.n_chunks;
+    a.tile_base = sl.b0; a.chunk_lo = sl.c0; a.chunk_hi = sl.c1;
+    a.seg_chunk = s.seg_chunk + sl.s0; a.seg_slot = s.seg_slot + sl.s0; a.n_segs = sl.s1 - sl.s0; a.out = s.out; a.seg_out = s.seg_out + sl.s0;
     a.rowq = e->d_rowq; a.rowq_count = e->d_rowq_count; a.rowq_cap = e->lim.rowq_cap; a.s = e->scratch;
     // the bulk path's first kernel empties the row queue; one call fewer on the host between the caller's enqueue and the kernels
     a.reset_rows = reset_rows && e->mode == 0 && a.n_segs ? 1u : 0u;
     if (reset_rows && !a.reset_rows) CK(e, cudaMemsetAsync(e->d_rowq_count, 0, 4, e->stream));
     int launched = 0;
-    const bool pk = e->per_kernel_timing || e->mode == 1;
-    cudaError_t r = launch_step(a, e->mode, e->sm_count, e->stream, e->ev, &launched, pk);
-    e->kernel_times_valid = pk;
+    const bool pk = e->step.per_kernel_timing || e->mode == 1;
+    cudaError_t r = launch_step(a, e->mode, e->sm_count, e->stream, e->step.ev, &launched, pk);
+    e->step.kernel_times_valid = pk;
     e->launches += (uint64_t)launched;
     if (r != cudaSuccess) { e->err = std::string("step launch: ") + cudaGetErrorString(r); return LGW_ERR_CUDA; }
-    e->timed = true;
+    e->step.timed = true;
     return LGW_OK;
 }
 
@@ -307,10 +371,10 @@ extern "C" int lgw_sse_step_device(lgw_engine* e, const uint8_t* d_bytes, uint64
                                    uint8_t* d_out, lgw_seg_result* d_seg_out) {
     if (!e || (!d_bytes && n_bytes) || !d_chunk_off || !d_seg_chunk || !d_seg_slot || (!d_out && n_bytes) || !d_seg_out) return LGW_ERR_ARG;
     CK(e, cudaSetDevice(e->device));
-    e->last_bytes = d_bytes; e->last_n_bytes = n_bytes; e->last_chunk_off = d_chunk_off; e->last_n_chunks = n_chunks;
-    e->last_seg_chunk = d_seg_chunk; e->last_seg_slot = d_seg_slot; e->last_n_segs = n_segs; e->last_seg_out = (const SegResult*)d_seg_out;
-    e->text_pending = e->text_on; e->text_ready = false;
-    return step_device(e, d_bytes, n_bytes, d_chunk_off, n_chunks, d_seg_chunk, d_seg_slot, n_segs, d_out, (SegResult*)d_seg_out);
+    const StepArrays s{d_bytes, n_bytes, d_chunk_off, n_chunks, d_seg_chunk, d_seg_slot, n_segs, d_out, (SegResult*)d_seg_out};
+    remember_step(e, s);
+    TRY(check_step_limits(e, n_segs, n_chunks, n_bytes));
+    return step_device(e, s, StepSlice::whole(n_segs, n_chunks, n_bytes), true);
 }
 
 extern "C" int lgw_fetch_rows(lgw_engine* e, lgw_row_event* rows_out, uint32_t rows_cap, uint32_t* n_rows) {
@@ -334,141 +398,149 @@ extern "C" int lgw_sync(lgw_engine* e) {
     return LGW_OK;
 }
 
+// cheap host-side validation of a host step's layout (offsets sorted, segments cover chunks in order)
+static int check_step_layout(lgw_engine* e, uint64_t n_bytes, const uint32_t* chunk_off, uint32_t n_chunks,
+                             const uint32_t* seg_chunk, const uint32_t* seg_slot, uint32_t n_segs) {
+    if (chunk_off[0] != 0 || chunk_off[n_chunks] != n_bytes) { e->err = "chunk_off must start at 0 and end at n_bytes"; return LGW_ERR_ARG; }
+    if (n_segs && (seg_chunk[0] != 0 || seg_chunk[n_segs] != n_chunks)) { e->err = "seg_chunk must cover all chunks"; return LGW_ERR_ARG; }
+    for (uint32_t s = 0; s < n_segs; ++s) if (seg_chunk[s] > seg_chunk[s + 1] || seg_slot[s] >= e->lim.max_streams) { e->err = "bad segment table"; return LGW_ERR_ARG; }
+    return LGW_OK;
+}
+
+// Host buffers that are page-locked (lgw_alloc_pinned, cudaHostAlloc, torch pin_memory) need no staging copy: the bulk kernel's
+// TMA loads can read the packed chunks straight from the host buffer ("direct in") and its TMA stores can write the re-emitted
+// bytes straight into the host output buffer ("direct out"); the parse of a tile then overlaps its own PCIe transfer.
+//   LGW_DIRECT = 0 (default) | in | out | both
+// The direct modes are correct and save the device staging buffers, but SM-issued PCIe traffic competes with the copy-engine
+// stream of the other direction, so the staged, sliced pipeline is the default.
+// Sets each pointer to the buffer's device address when that direction may run direct, else to null.
+static void probe_direct(const lgw_engine* e, const uint8_t* bytes, uint8_t* out_bytes, uint64_t n_bytes, const uint8_t** direct_in, uint8_t** direct_out) {
+    static const int allow = [] { const char* v = getenv("LGW_DIRECT"); if (!v || v[0] == '0') return 0; if (v[0] == 'b') return 3; if (v[0] == 'o') return 2; return 1; }();
+    cudaPointerAttributes pa{};
+    const bool big = e->mode == 0 && n_bytes >= (1u << 20);
+    *direct_in = nullptr; *direct_out = nullptr;
+    if (big && (allow & 1) && ((uintptr_t)bytes & 15) == 0 && cudaPointerGetAttributes(&pa, bytes) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer)
+        *direct_in = (const uint8_t*)pa.devicePointer;
+    if (big && out_bytes && (allow & 2) && ((uintptr_t)out_bytes & 15) == 0 && cudaPointerGetAttributes(&pa, out_bytes) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer)
+        *direct_out = (uint8_t*)pa.devicePointer;
+    cudaGetLastError();                 // (cudaPointerGetAttributes on an unregistered pointer may leave an error behind)
+}
+
+// The step is cut at segment boundaries into slices so that whatever goes through the copy engines overlaps with the kernels:
+// upload of slice k+1 | kernels of slice k | download of slice k-1 (PCIe is full duplex).   LGW_SLICES = 1..14
+static uint32_t choose_slices(const lgw_engine* e, uint64_t n_bytes, uint32_t n_segs, bool all_direct) {
+    uint32_t n_slices = n_bytes >= (8u << 20) && n_segs >= 16 ? 8u : 1u;
+    if (all_direct) n_slices = 1;
+    if (const char* sl = getenv("LGW_SLICES")) { int v = atoi(sl); if (v >= 1 && v <= 14) n_slices = (uint32_t)v; }
+    if (e->mode == 1) n_slices = 1;
+    return n_slices;
+}
+
+// LGW_TRACE = 1: the slice timeline of the step that just ran.  A slice without segments ran nothing and prints -1.
+static void print_trace(lgw_engine* e, bool direct_in, bool direct_out, const uint32_t* cut, uint32_t n_slices) {
+    cudaDeviceSynchronize();
+    fprintf(stderr, "[lgw trace] direct_in=%d direct_out=%d slices=%u total=%.3f ms; per slice (ms after step start): upload done | kernels done | download done\n", direct_in, direct_out, n_slices, e->step.ms[4]);
+    for (uint32_t j = 0; j < n_slices; ++j) {
+        float ms[3] = {-1, -1, -1};
+        if (cut[j + 1] > cut[j] || n_slices == 1) for (int k = 0; k < 3; ++k) read_ms(e->step.ev[5], e->step.tr[k][j], ms[k]);
+        fprintf(stderr, "[lgw trace]   %2u  %.3f | %.3f | %.3f\n", j, ms[0], ms[1], ms[2]);
+    }
+    cudaGetLastError();
+}
+
 extern "C" int lgw_sse_step(lgw_engine* e, const uint8_t* bytes, uint64_t n_bytes, const uint32_t* chunk_off, uint32_t n_chunks,
                             const uint32_t* seg_chunk, const uint32_t* seg_slot, uint32_t n_segs,
                             uint8_t* out_bytes, lgw_seg_result* seg_out, lgw_row_event* rows_out, uint32_t rows_cap, uint32_t* n_rows) {
     if (!e || (!bytes && n_bytes) || !chunk_off || !seg_chunk || !seg_slot || !seg_out || !n_rows) return LGW_ERR_ARG;
     // out_bytes == NULL: the caller relays its own copy of the chunk bytes (the relayed bytes ARE the original bytes, request_handler.py:141-142);
     // the kernels run unchanged (the re-emit lands in the device staging buffer), only the download of the bytes is left out
-    if (n_segs > e->lim.max_streams || n_chunks > e->lim.max_step_chunks || n_bytes > e->lim.max_step_bytes) {
-        e->err = "step exceeds the limits given to lgw_engine_create"; return LGW_ERR_CAPACITY;
-    }
-    // cheap host-side validation of the layout (offsets sorted, segments cover chunks in order)
-    if (chunk_off[0] != 0 || chunk_off[n_chunks] != n_bytes) { e->err = "chunk_off must start at 0 and end at n_bytes"; return LGW_ERR_ARG; }
-    if (n_segs && (seg_chunk[0] != 0 || seg_chunk[n_segs] != n_chunks)) { e->err = "seg_chunk must cover all chunks"; return LGW_ERR_ARG; }
-    for (uint32_t s = 0; s < n_segs; ++s) if (seg_chunk[s] > seg_chunk[s + 1] || seg_slot[s] >= e->lim.max_streams) { e->err = "bad segment table"; return LGW_ERR_ARG; }
+    TRY(check_step_limits(e, n_segs, n_chunks, n_bytes));
+    TRY(check_step_layout(e, n_bytes, chunk_off, n_chunks, seg_chunk, seg_slot, n_segs));
+    lgw_engine::Step& st = e->step;
     CK(e, cudaSetDevice(e->device));
-    CK(e, cudaEventRecord(e->ev[5], e->stream));
-    // Host buffers that are page-locked (lgw_alloc_pinned, cudaHostAlloc, torch pin_memory) need no staging copy: the bulk kernel's
-    // TMA loads can read the packed chunks straight from the host buffer ("direct in") and its TMA stores can write the re-emitted
-    // bytes straight into the host output buffer ("direct out"); the parse of a tile then overlaps its own PCIe transfer.  The
-    // step is cut at segment boundaries into slices so that whatever still goes through the copy engines (the other direction)
-    // overlaps with the kernels: upload of slice k+1 | kernels of slice k | download of slice k-1 (PCIe is full duplex).
-    //   LGW_DIRECT = 0 (default) | in | out | both        LGW_SLICES = 1..14        LGW_TRACE = 1 prints the slice timeline
-    // The direct modes are correct and save the device staging buffers, but SM-issued PCIe traffic competes with the copy-engine
-    // stream of the other direction, so the staged, sliced pipeline is the default.
-    static const int allow = [] { const char* v = getenv("LGW_DIRECT"); if (!v || v[0] == '0') return 0; if (v[0] == 'b') return 3; if (v[0] == 'o') return 2; return 1; }();
+    CK(e, cudaEventRecord(st.ev[5], e->stream));
     static const bool trace = [] { const char* v = getenv("LGW_TRACE"); return v && v[0] == '1'; }();
-    const uint8_t* direct_in = nullptr; uint8_t* direct_out = nullptr;
-    {
-        cudaPointerAttributes pa{};
-        const bool big = e->mode == 0 && n_bytes >= (1u << 20);
-        if (big && (allow & 1) && ((uintptr_t)bytes & 15) == 0 && cudaPointerGetAttributes(&pa, bytes) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer)
-            direct_in = (const uint8_t*)pa.devicePointer;
-        if (big && out_bytes && (allow & 2) && ((uintptr_t)out_bytes & 15) == 0 && cudaPointerGetAttributes(&pa, out_bytes) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer)
-            direct_out = (uint8_t*)pa.devicePointer;
-        cudaGetLastError();                 // (cudaPointerGetAttributes on an unregistered pointer may leave an error behind)
-        e->last_direct = direct_in || direct_out;
-    }
-    e->last_bytes = direct_in ? direct_in : e->d_in; e->last_n_bytes = n_bytes; e->last_chunk_off = e->d_chunk_off; e->last_n_chunks = n_chunks;
-    e->last_seg_chunk = e->d_seg_chunk; e->last_seg_slot = e->d_seg_slot; e->last_n_segs = n_segs; e->last_seg_out = e->d_seg_out;
-    e->text_pending = e->text_on; e->text_ready = false;
-    uint32_t n_slices = n_bytes >= (8u << 20) && n_segs >= 16 ? 8u : 1u;
-    if (direct_in && direct_out) n_slices = 1;
-    if (const char* sl = getenv("LGW_SLICES")) { int v = atoi(sl); if (v >= 1 && v <= 14) n_slices = (uint32_t)v; }
-    if (e->mode == 1) n_slices = 1;
+    const uint8_t* direct_in; uint8_t* direct_out;
+    probe_direct(e, bytes, out_bytes, n_bytes, &direct_in, &direct_out);
+    st.last_direct = direct_in || direct_out;
+    const StepArrays dev{direct_in ? direct_in : st.d_in, n_bytes, st.d_chunk_off, n_chunks, st.d_seg_chunk, st.d_seg_slot, n_segs,
+                         direct_out ? direct_out : st.d_out, st.d_seg_out};
+    remember_step(e, dev);
     uint32_t cut[18];
-    n_slices = step_slice_cuts(n_bytes, chunk_off, seg_chunk, n_segs, n_slices, cut);
+    const uint32_t n_slices = step_slice_cuts(n_bytes, chunk_off, seg_chunk, n_segs, choose_slices(e, n_bytes, n_segs, direct_in && direct_out), cut);
     CK(e, cudaMemsetAsync(e->d_rowq_count, 0, 4, e->stream));
     const bool piped = n_slices > 1;
     cudaStream_t sin = piped ? e->s_in : e->stream, sout = piped ? e->s_out : e->stream;
-    if (piped) { CK(e, cudaEventRecord(e->ev_k[15], e->stream)); CK(e, cudaStreamWaitEvent(sin, e->ev_k[15], 0)); }   // the copy stream starts after ev[5]
+    if (piped) { CK(e, cudaEventRecord(st.ev_k[15], e->stream)); CK(e, cudaStreamWaitEvent(sin, st.ev_k[15], 0)); }   // the copy stream starts after ev[5]
     // offsets and segment tables: slice 0's part first (its kernels can start), everything else in one batch right behind it
-    {
-        const uint32_t s1 = cut[1], c1 = seg_chunk[s1];
-        CK(e, cudaMemcpyAsync(e->d_chunk_off, chunk_off, (size_t)(c1 + 1) * 4, cudaMemcpyHostToDevice, sin));
-        CK(e, cudaMemcpyAsync(e->d_seg_chunk, seg_chunk, (size_t)(n_segs + 1) * 4, cudaMemcpyHostToDevice, sin));
-        if (n_segs) CK(e, cudaMemcpyAsync(e->d_seg_slot, seg_slot, (size_t)n_segs * 4, cudaMemcpyHostToDevice, sin));
-    }
-    cudaEvent_t tr[3][16]; float tms[3][16];
-    if (trace) for (int k = 0; k < 3; ++k) for (uint32_t j = 0; j < n_slices; ++j) cudaEventCreate(&tr[k][j]);
-    int rc = LGW_OK;
+    CK(e, cudaMemcpyAsync(st.d_chunk_off, chunk_off, (size_t)(seg_chunk[cut[1]] + 1) * 4, cudaMemcpyHostToDevice, sin));
+    CK(e, cudaMemcpyAsync(st.d_seg_chunk, seg_chunk, (size_t)(n_segs + 1) * 4, cudaMemcpyHostToDevice, sin));
+    if (n_segs) CK(e, cudaMemcpyAsync(st.d_seg_slot, seg_slot, (size_t)n_segs * 4, cudaMemcpyHostToDevice, sin));
+    if (trace && !st.tr[0][0]) CK(e, new_events(e, &st.tr[0][0], 3 * 16));
     for (uint32_t j = 0; j < n_slices; ++j) {
         const uint32_t s0 = cut[j], s1 = cut[j + 1];
         if (s1 <= s0 && piped) continue;
         const uint32_t c0 = seg_chunk[s0], c1 = seg_chunk[s1];
         const uint32_t b0 = chunk_off[c0]; const uint64_t b1 = chunk_off[c1];
-        if (!direct_in && b1 > b0) CK(e, cudaMemcpyAsync(e->d_in + b0, bytes + b0, b1 - b0, cudaMemcpyHostToDevice, sin));
-        if (piped && (j == 0 || !direct_in)) { CK(e, cudaEventRecord(e->ev_in[j], sin)); CK(e, cudaStreamWaitEvent(e->stream, e->ev_in[j], 0)); }
-        if (trace) cudaEventRecord(tr[0][j], sin);
+        if (!direct_in && b1 > b0) CK(e, cudaMemcpyAsync(st.d_in + b0, bytes + b0, b1 - b0, cudaMemcpyHostToDevice, sin));
+        if (piped && (j == 0 || !direct_in)) { CK(e, cudaEventRecord(st.ev_in[j], sin)); CK(e, cudaStreamWaitEvent(e->stream, st.ev_in[j], 0)); }
+        if (trace) cudaEventRecord(st.tr[0][j], sin);
         if (j == 0 && n_slices > 1 && n_chunks > seg_chunk[cut[1]]) {      // the rest of the chunk offsets, while slice 0 is at work
             const uint32_t cc = seg_chunk[cut[1]];
-            CK(e, cudaMemcpyAsync(e->d_chunk_off + cc + 1, chunk_off + cc + 1, (size_t)(n_chunks - cc) * 4, cudaMemcpyHostToDevice, sin));
-            if (direct_in) { CK(e, cudaEventRecord(e->ev_in[1], sin)); CK(e, cudaStreamWaitEvent(e->stream, e->ev_in[1], 0)); }
+            CK(e, cudaMemcpyAsync(st.d_chunk_off + cc + 1, chunk_off + cc + 1, (size_t)(n_chunks - cc) * 4, cudaMemcpyHostToDevice, sin));
+            if (direct_in) { CK(e, cudaEventRecord(st.ev_in[1], sin)); CK(e, cudaStreamWaitEvent(e->stream, st.ev_in[1], 0)); }
         }
-        rc = step_device(e, direct_in ? direct_in : e->d_in, n_bytes, e->d_chunk_off, n_chunks, e->d_seg_chunk, e->d_seg_slot, n_segs,
-                         direct_out ? direct_out : e->d_out, e->d_seg_out, s0, s1, c0, c1, b0, b1, false);
-        if (rc != LGW_OK) return rc;
-        if (trace) cudaEventRecord(tr[1][j], e->stream);
+        TRY(step_device(e, dev, StepSlice{s0, s1, c0, c1, b0, b1}, false));
+        if (trace) cudaEventRecord(st.tr[1][j], e->stream);
         if (!direct_out) {
-            if (piped) { CK(e, cudaEventRecord(e->ev_k[j], e->stream)); CK(e, cudaStreamWaitEvent(sout, e->ev_k[j], 0)); }
-            if (b1 > b0 && out_bytes) CK(e, cudaMemcpyAsync(out_bytes + b0, e->d_out + b0, b1 - b0, cudaMemcpyDeviceToHost, sout));
+            if (piped) { CK(e, cudaEventRecord(st.ev_k[j], e->stream)); CK(e, cudaStreamWaitEvent(sout, st.ev_k[j], 0)); }
+            if (b1 > b0 && out_bytes) CK(e, cudaMemcpyAsync(out_bytes + b0, st.d_out + b0, b1 - b0, cudaMemcpyDeviceToHost, sout));
         }
-        if (trace) cudaEventRecord(tr[2][j], sout);
+        if (trace) cudaEventRecord(st.tr[2][j], sout);
     }
     // per-segment results: one copy at the end (a copy into pageable host memory blocks the host thread,
     // which would serialise the pipeline if it were issued per slice)
-    if (n_segs) CK(e, cudaMemcpyAsync(seg_out, e->d_seg_out, (size_t)n_segs * sizeof(SegResult), cudaMemcpyDeviceToHost, e->stream));
+    if (n_segs) CK(e, cudaMemcpyAsync(seg_out, st.d_seg_out, (size_t)n_segs * sizeof(SegResult), cudaMemcpyDeviceToHost, e->stream));
     if (piped) {                            // ev[6] closes the step on the engine stream: it has to see the downloads too
-        CK(e, cudaEventRecord(e->ev_k[14], sout)); CK(e, cudaStreamWaitEvent(e->stream, e->ev_k[14], 0));
-        CK(e, cudaEventRecord(e->ev_in[15], sin)); CK(e, cudaStreamWaitEvent(e->stream, e->ev_in[15], 0));
+        CK(e, cudaEventRecord(st.ev_k[14], sout)); CK(e, cudaStreamWaitEvent(e->stream, st.ev_k[14], 0));
+        CK(e, cudaEventRecord(st.ev_in[15], sin)); CK(e, cudaStreamWaitEvent(e->stream, st.ev_in[15], 0));
     }
-    CK(e, cudaEventRecord(e->ev[6], e->stream));
-    rc = lgw_fetch_rows(e, rows_out, rows_cap, n_rows);
-    if (rc != LGW_OK) return rc;
+    CK(e, cudaEventRecord(st.ev[6], e->stream));
+    TRY(lgw_fetch_rows(e, rows_out, rows_cap, n_rows));
     if (piped) { CK(e, cudaStreamSynchronize(e->s_out)); CK(e, cudaStreamSynchronize(e->s_in)); }
-    float t = 0; if (cudaEventElapsedTime(&t, e->ev[5], e->ev[6]) == cudaSuccess) e->ms[4] = t;
-    if (trace) {
-        cudaDeviceSynchronize();
-        fprintf(stderr, "[lgw trace] direct_in=%d direct_out=%d slices=%u total=%.3f ms; per slice (ms after step start): upload done | kernels done | download done\n", direct_in != nullptr, direct_out != nullptr, n_slices, t);
-        for (uint32_t j = 0; j < n_slices; ++j) {
-            for (int k = 0; k < 3; ++k) { tms[k][j] = -1; cudaEventElapsedTime(&tms[k][j], e->ev[5], tr[k][j]); cudaEventDestroy(tr[k][j]); }
-            fprintf(stderr, "[lgw trace]   %2u  %.3f | %.3f | %.3f\n", j, tms[0][j], tms[1][j], tms[2][j]);
-        }
-        cudaGetLastError();
-    }
+    read_ms(st.ev[5], st.ev[6], st.ms[4]);
+    if (trace) print_trace(e, direct_in != nullptr, direct_out != nullptr, cut, n_slices);
     return LGW_OK;
 }
 
 static int read_step_ms(lgw_engine* e) {
-    if (e->timed) {
+    lgw_engine::Step& st = e->step;
+    if (st.timed) {
         CK(e, cudaSetDevice(e->device));
-        CK(e, cudaEventSynchronize(e->ev[4]));
-        if (e->kernel_times_valid) {
-            for (int i = 0; i < 4; ++i) { float t = 0; if (cudaEventElapsedTime(&t, e->ev[i], e->ev[i + 1]) == cudaSuccess) e->ms[i] = t; }
+        CK(e, cudaEventSynchronize(st.ev[4]));
+        if (st.kernel_times_valid) {
+            for (int i = 0; i < 4; ++i) read_ms(st.ev[i], st.ev[i + 1], st.ms[i]);
         } else {                            // kernels overlap (programmatic dependent launch): only their total is meaningful
-            float t = 0; e->ms[0] = e->ms[2] = e->ms[3] = 0;
-            if (cudaEventElapsedTime(&t, e->ev[0], e->ev[4]) == cudaSuccess) e->ms[1] = t;
+            st.ms[0] = st.ms[2] = st.ms[3] = 0;
+            read_ms(st.ev[0], st.ev[4], st.ms[1]);
         }
     }
     return LGW_OK;
 }
 extern "C" int lgw_last_step_ms(lgw_engine* e, float ms[4]) {
     if (!e || !ms) return LGW_ERR_ARG;
-    const int rc = read_step_ms(e);
-    if (rc != LGW_OK) return rc;
-    ms[0] = e->ms[0]; ms[1] = e->ms[1]; ms[2] = e->ms[2] + e->ms[3]; ms[3] = e->ms[4];
+    TRY(read_step_ms(e));
+    ms[0] = e->step.ms[0]; ms[1] = e->step.ms[1]; ms[2] = e->step.ms[2] + e->step.ms[3]; ms[3] = e->step.ms[4];
     return LGW_OK;
 }
 extern "C" int lgw_last_step_kernel_ms(lgw_engine* e, float ms[4]) {
     if (!e || !ms) return LGW_ERR_ARG;
-    const int rc = read_step_ms(e);
-    if (rc != LGW_OK) return rc;
-    for (int i = 0; i < 4; ++i) ms[i] = e->ms[i];
+    TRY(read_step_ms(e));
+    for (int i = 0; i < 4; ++i) ms[i] = e->step.ms[i];
     return LGW_OK;
 }
 
-extern "C" int lgw_last_step_direct(lgw_engine* e) { return e && e->last_direct ? 1 : 0; }
+extern "C" int lgw_last_step_direct(lgw_engine* e) { return e && e->step.last_direct ? 1 : 0; }
 
 extern "C" int lgw_launch_count(lgw_engine* e, uint64_t* out) {
     if (!e || !out) return LGW_ERR_ARG;
@@ -476,6 +548,7 @@ extern "C" int lgw_launch_count(lgw_engine* e, uint64_t* out) {
     return LGW_OK;
 }
 
+// Page-locked host memory is the caller's until lgw_free_pinned: the engine keeps no record of it.
 extern "C" int lgw_alloc_pinned(lgw_engine* e, uint64_t bytes, void** out) {
     if (!e || !out) return LGW_ERR_ARG;
     CK(e, cudaSetDevice(e->device));
@@ -505,6 +578,7 @@ extern "C" int lgw_usage_rollup_accum(lgw_engine* e, const int64_t* d_ts_us, con
     if (!e || !d_table || !d_inexact || !d_oob || period < 0 || period > 3 || n_buckets == 0 || n_models == 0) return LGW_ERR_ARG;
     if (n && (!d_ts_us || !d_model_rank || !d_prompt || !d_completion || !d_total || !d_reasoning || !d_cached || !d_cost)) return LGW_ERR_ARG;
     CK(e, cudaSetDevice(e->device));
+    lgw_engine::Rollup& ru = e->rollup;
     RollupArgs a{};
     a.ts_us = d_ts_us; a.model_rank = d_model_rank; a.tok[0] = d_prompt; a.tok[1] = d_completion; a.tok[2] = d_total;
     a.tok[3] = d_reasoning; a.tok[4] = d_cached; a.cost = d_cost; a.n = n; a.period = period;
@@ -512,34 +586,27 @@ extern "C" int lgw_usage_rollup_accum(lgw_engine* e, const int64_t* d_ts_us, con
     a.bucket0 = bucket0; a.n_buckets = n_buckets; a.n_models = n_models;
     a.table = (unsigned long long*)d_table; a.inexact = d_inexact; a.oob = d_oob;
     const uint64_t groups = (uint64_t)n_buckets * n_models;
-    const bool privatised = groups <= LGW_ROLLUP_SMEM_GROUPS && n >= 65536 && n < 0xFFFFFFFFull && !e->rollup_force_global;
+    const bool privatised = groups <= LGW_ROLLUP_SMEM_GROUPS && n >= 65536 && n < 0xFFFFFFFFull && !ru.force_global;
     if (privatised) {                     // scratch for the per-block partial tables (allocated outside the timed region)
-        const size_t need = (size_t)e->sm_count * groups * (LGW_ROLLUP_CELLS * 8 + 4);
-        if (need > e->d_partial_cap) {
-            cudaFree(e->d_partial); e->d_partial = nullptr; e->d_partial_cap = 0;
-            CK(e, cudaMalloc((void**)&e->d_partial, need));
-            e->d_partial_cap = need;
-        }
-        if (!e->rollup_attr_set) {
+        CK(e, ru.partial.reserve((size_t)e->sm_count * groups * (LGW_ROLLUP_CELLS * 8 + 4)));
+        if (!ru.attr_set) {
             CK(e, cudaFuncSetAttribute(k_rollup_accum_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rollup_smem_bytes(LGW_ROLLUP_SMEM_GROUPS)));
-            e->rollup_attr_set = true;
+            ru.attr_set = true;
         }
     }
-    CK(e, cudaEventRecord(e->rev[0], e->stream));
+    CK(e, cudaEventRecord(ru.ev[0], e->stream));
     if (n && privatised) {
         const unsigned grid = (unsigned)e->sm_count;
-        unsigned long long* partial = (unsigned long long*)e->d_partial;
-        uint32_t* pflag = (uint32_t*)(e->d_partial + (size_t)grid * groups * LGW_ROLLUP_CELLS * 8);
+        unsigned long long* partial = ru.partial.as<unsigned long long>();
+        uint32_t* pflag = (uint32_t*)(ru.partial.as<uint8_t>() + (size_t)grid * groups * LGW_ROLLUP_CELLS * 8);
         k_rollup_accum_smem<<<grid, 1024, rollup_smem_bytes((uint32_t)groups), e->stream>>>(a, partial, pflag);
         k_rollup_merge<<<dim3((unsigned)((groups * LGW_ROLLUP_CELLS + 255) / 256), LGW_ROLLUP_MERGE_SLICES), 256, 0, e->stream>>>(partial, pflag, grid, (uint32_t)groups, a.table, a.inexact);
         e->launches += 2;
     } else if (n) {
-        const uint64_t want = (n + 255) / 256;
-        const unsigned grid = (unsigned)(want < (uint64_t)e->sm_count * 16 ? want : (uint64_t)e->sm_count * 16);
-        k_rollup_accum<<<grid, 256, 0, e->stream>>>(a);
+        k_rollup_accum<<<grid_for(e, n, 256, 16), 256, 0, e->stream>>>(a);
         ++e->launches;
     }
-    CK(e, cudaEventRecord(e->rev[1], e->stream));
+    CK(e, cudaEventRecord(ru.ev[1], e->stream));
     CK(e, cudaGetLastError());
     return LGW_OK;
 }
@@ -549,51 +616,44 @@ extern "C" int lgw_usage_rollup_emit(lgw_engine* e, const uint64_t* d_table, con
                                      lgw_rollup_row* rows_out, uint64_t rows_cap, uint64_t* n_rows) {
     if (!e || !d_table || !d_inexact || !n_rows || (!rows_out && rows_cap) || n_buckets == 0 || n_models == 0) return LGW_ERR_ARG;
     CK(e, cudaSetDevice(e->device));
+    lgw_engine::Rollup& ru = e->rollup;
     const uint64_t groups = (uint64_t)n_buckets * n_models;
     const uint64_t cap = rows_cap < groups ? rows_cap : groups;
-    if (cap > e->d_rows_cap) {
-        cudaFree(e->d_rows); e->d_rows = nullptr; e->d_rows_cap = 0;
-        CK(e, cudaMalloc((void**)&e->d_rows, (cap ? cap : 1) * sizeof(RollupRow)));
-        e->d_rows_cap = cap;
-    }
-    if (!e->d_nrows) CK(e, cudaMalloc((void**)&e->d_nrows, 8));
+    CK(e, ru.rows.reserve(cap * sizeof(RollupRow)));
+    if (!ru.d_nrows) CK(e, dev_alloc(e, ru.d_nrows, 8));
     const uint32_t n_tiles = (uint32_t)((groups + 1023) / 1024);
-    if (n_tiles > e->d_tiles_cap) {
-        cudaFree(e->d_tiles); e->d_tiles = nullptr; e->d_tiles_cap = 0;
-        CK(e, cudaMalloc((void**)&e->d_tiles, (size_t)n_tiles * 4));
-        e->d_tiles_cap = n_tiles;
-    }
-    CK(e, cudaEventRecord(e->rev[2], e->stream));
-    k_rollup_count<<<n_tiles, 1024, 0, e->stream>>>((const unsigned long long*)d_table, n_buckets, n_models, e->d_tiles);
-    k_rollup_scan<<<1, 1024, 0, e->stream>>>(e->d_tiles, n_tiles, e->d_nrows);
-    k_rollup_write<<<n_tiles, 1024, 0, e->stream>>>((const unsigned long long*)d_table, d_inexact, n_buckets, n_models, bucket0, e->d_tiles, e->d_rows, cap);
+    CK(e, ru.tiles.reserve((size_t)n_tiles * 4));
+    CK(e, cudaEventRecord(ru.ev[2], e->stream));
+    k_rollup_count<<<n_tiles, 1024, 0, e->stream>>>((const unsigned long long*)d_table, n_buckets, n_models, ru.tiles.as<uint32_t>());
+    k_rollup_scan<<<1, 1024, 0, e->stream>>>(ru.tiles.as<uint32_t>(), n_tiles, ru.d_nrows);
+    k_rollup_write<<<n_tiles, 1024, 0, e->stream>>>((const unsigned long long*)d_table, d_inexact, n_buckets, n_models, bucket0, ru.tiles.as<uint32_t>(), ru.rows.as<RollupRow>(), cap);
     e->launches += 3;
-    CK(e, cudaEventRecord(e->rev[3], e->stream));
+    CK(e, cudaEventRecord(ru.ev[3], e->stream));
     CK(e, cudaGetLastError());
     unsigned long long cnt = 0;
-    CK(e, cudaMemcpyAsync(&cnt, e->d_nrows, 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(&cnt, ru.d_nrows, 8, cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     *n_rows = cnt;
     const uint64_t take = cnt < cap ? cnt : cap;
-    if (take) CK(e, cudaMemcpyAsync(rows_out, e->d_rows, take * sizeof(RollupRow), cudaMemcpyDeviceToHost, e->stream));
+    if (take) CK(e, cudaMemcpyAsync(rows_out, ru.rows.p, take * sizeof(RollupRow), cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     return LGW_OK;
 }
 
 extern "C" int lgw_rollup_set_path(lgw_engine* e, int force_global) {   // 0 (default): privatised when the table fits; 1: global reductions only
     if (!e) return LGW_ERR_ARG;
-    e->rollup_force_global = force_global != 0;
+    e->rollup.force_global = force_global != 0;
     return LGW_OK;
 }
 
 extern "C" int lgw_rollup_last_ms(lgw_engine* e, float ms[2]) {
     if (!e || !ms) return LGW_ERR_ARG;
     CK(e, cudaSetDevice(e->device));
-    cudaEventSynchronize(e->rev[1]); cudaEventSynchronize(e->rev[3]);
-    float t = 0;
-    if (cudaEventElapsedTime(&t, e->rev[0], e->rev[1]) == cudaSuccess) e->rms[0] = t;
-    if (cudaEventElapsedTime(&t, e->rev[2], e->rev[3]) == cudaSuccess) e->rms[1] = t;
-    ms[0] = e->rms[0]; ms[1] = e->rms[1];
+    lgw_engine::Rollup& ru = e->rollup;
+    cudaEventSynchronize(ru.ev[1]); cudaEventSynchronize(ru.ev[3]);
+    read_ms(ru.ev[0], ru.ev[1], ru.ms[0]);
+    read_ms(ru.ev[2], ru.ev[3], ru.ms[1]);
+    ms[0] = ru.ms[0]; ms[1] = ru.ms[1];
     return LGW_OK;
 }
 
@@ -601,7 +661,8 @@ extern "C" int lgw_rollup_last_ms(lgw_engine* e, float ms[2]) {
 extern "C" int lgw_usage_latest(lgw_engine* e, const int64_t* d_ts_us, uint64_t n, uint64_t first, uint64_t count, uint64_t* idx_out) {
     if (!e || n >= (1ull << 32) || count > n || first > n - count) return LGW_ERR_ARG;
     if (count && (!d_ts_us || !idx_out || ((uintptr_t)d_ts_us & 15))) return LGW_ERR_ARG;
-    e->lms = 0;
+    lgw_engine::Listing& li = e->listing;
+    li.ms = 0;
     if (!count) return LGW_OK;
     CK(e, cudaSetDevice(e->device));
     const uint32_t N = (uint32_t)n, M = (uint32_t)count, cap = N / LGW_LIST_CAND_DIV;
@@ -610,28 +671,23 @@ extern "C" int lgw_usage_latest(lgw_engine* e, const int64_t* d_ts_us, uint64_t 
     auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
     const size_t o_cand = al(sizeof(ListSel)), o_keys = o_cand + al((size_t)(cap ? cap : 1) * sizeof(ListPair));
     const size_t o_idx = o_keys + al((size_t)M * 16), o_out = o_idx + al((size_t)M * 8), o_scan = o_out + al((size_t)M * 8);
-    const size_t need = o_scan + al((scan_n + 257) * 4);
-    if (need > e->l_cap) {
-        cudaFree(e->l_buf); e->l_buf = nullptr; e->l_cap = 0;
-        CK(e, cudaMalloc((void**)&e->l_buf, need));
-        e->l_cap = need;
-    }
-    if (!e->lev[0]) for (auto& ev : e->lev) CK(e, cudaEventCreate(&ev));
-    if (!e->list_attr_set) {
+    CK(e, li.buf.reserve(o_scan + al((scan_n + 257) * 4)));
+    if (!li.ev[0]) CK(e, new_events(e, li.ev, 2));
+    if (!li.attr_set) {
         CK(e, cudaFuncSetAttribute(k_list_sort_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(LGW_LIST_SMEM_SORT * 12)));
-        e->list_attr_set = true;
+        li.attr_set = true;
     }
-    ListSel* sel = (ListSel*)e->l_buf;
-    ListPair* cand = (ListPair*)(e->l_buf + o_cand);
-    uint64_t* keys[2] = {(uint64_t*)(e->l_buf + o_keys), (uint64_t*)(e->l_buf + o_keys) + M};
-    uint32_t* idx[2] = {(uint32_t*)(e->l_buf + o_idx), (uint32_t*)(e->l_buf + o_idx) + M};
-    uint64_t* out = (uint64_t*)(e->l_buf + o_out);
-    uint32_t* scan = (uint32_t*)(e->l_buf + o_scan);
+    uint8_t* l_buf = li.buf.as<uint8_t>();
+    ListSel* sel = (ListSel*)l_buf;
+    ListPair* cand = (ListPair*)(l_buf + o_cand);
+    uint64_t* keys[2] = {(uint64_t*)(l_buf + o_keys), (uint64_t*)(l_buf + o_keys) + M};
+    uint32_t* idx[2] = {(uint32_t*)(l_buf + o_idx), (uint32_t*)(l_buf + o_idx) + M};
+    uint64_t* out = (uint64_t*)(l_buf + o_out);
+    uint32_t* scan = (uint32_t*)(l_buf + o_scan);
     uint32_t* totals = scan + scan_n;                   // [256] column totals of the LSD scans
     uint32_t* selected = totals + 256;                  // records between the two boundaries (== count)
-    const uint32_t pairs = (uint32_t)(((uint64_t)N + 1) / 2);
-    const uint32_t want = (pairs + 255) / 256, grid = want < (uint32_t)e->sm_count * 8 ? want : (uint32_t)e->sm_count * 8;
-    CK(e, cudaEventRecord(e->lev[0], e->stream));
+    const unsigned grid = grid_for(e, ((uint64_t)N + 1) / 2, 256, 8);
+    CK(e, cudaEventRecord(li.ev[0], e->stream));
     k_list_init<<<1, 256, 0, e->stream>>>(sel, first, first + count - 1);
     for (int d = 0; d < LGW_LIST_DIGITS; ++d) {
         k_list_hist<<<grid, 256, 0, e->stream>>>(d_ts_us, N, cand, sel, d);
@@ -654,102 +710,105 @@ extern "C" int lgw_usage_latest(lgw_engine* e, const int64_t* d_ts_us, uint64_t 
             k_list_scan<<<256, 1024, 0, e->stream>>>(scan, stiles, totals);
             k_lsd_scatter<<<stiles, 256, 0, e->stream>>>(keys[cur], idx[cur], M, shift, scan, totals, stiles, keys[cur ^ 1], idx[cur ^ 1]);
         }
-        const uint32_t wg = (M + 255) / 256 < (uint32_t)e->sm_count * 8 ? (M + 255) / 256 : (uint32_t)e->sm_count * 8;
-        k_list_widen<<<wg, 256, 0, e->stream>>>(idx[cur], M, out);
+        k_list_widen<<<grid_for(e, M, 256, 8), 256, 0, e->stream>>>(idx[cur], M, out);
         e->launches += 8 * 3 + 1;
     }
-    CK(e, cudaEventRecord(e->lev[1], e->stream));
+    CK(e, cudaEventRecord(li.ev[1], e->stream));
     CK(e, cudaGetLastError());
     uint32_t got = 0;
     CK(e, cudaMemcpyAsync(idx_out, out, (size_t)M * 8, cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaMemcpyAsync(&got, selected, 4, cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
-    float t = 0;
-    if (cudaEventElapsedTime(&t, e->lev[0], e->lev[1]) == cudaSuccess) e->lms = t;
+    read_ms(li.ev[0], li.ev[1], li.ms);
     if (got != M) { e->err = "usage listing: " + std::to_string(got) + " records between the boundary keys, expected " + std::to_string(M); return LGW_ERR_CUDA; }
     return LGW_OK;
 }
 
 extern "C" int lgw_usage_latest_last_ms(lgw_engine* e, float* ms) {
     if (!e || !ms) return LGW_ERR_ARG;
-    *ms = e->lms;
+    *ms = e->listing.ms;
     return LGW_OK;
 }
 
 // ---- transcript tap (SURVEY.md 8(f) rank 3; chat_logging.py:108-139) ---------------------------------------------------------
 extern "C" int lgw_transcripts_enable(lgw_engine* e) {
     if (!e) return LGW_ERR_ARG;
-    if (e->text_on) return LGW_OK;
+    lgw_engine::Text& tx = e->text;
+    if (tx.on) return LGW_OK;
     CK(e, cudaSetDevice(e->device));
     const size_t S = e->lim.max_streams, C = e->lim.max_step_chunks, B = e->lim.max_step_bytes, cc = e->lim.carry_cap;
-    CK(e, cudaMalloc((void**)&e->d_tap, S * sizeof(TextTap)));
-    CK(e, cudaMemset(e->d_tap, 0, S * sizeof(TextTap)));
-    CK(e, cudaMalloc((void**)&e->d_tcarry, S * cc));
-    CK(e, cudaMalloc((void**)&e->d_tsparse, 2 * (B + S * cc) + 64));  // per segment: twice its carry and its bytes (content pieces + "error" event texts)
-    CK(e, cudaMalloc((void**)&e->d_ttext, 2 * (B + S * cc) + 64));
-    CK(e, cudaMalloc((void**)&e->d_piece_len, (C + 1) * 4));
-    CK(e, cudaMalloc((void**)&e->d_tseg_len, (S + 1) * 4));
-    CK(e, cudaMalloc((void**)&e->d_tseg_flags, (S + 1) * 4));
-    CK(e, cudaMalloc((void**)&e->d_tseg_off, (S + 2) * 8));
-    CK(e, cudaMalloc((void**)&e->d_markq, (size_t)(e->lim.rowq_cap + 1) * sizeof(TextMark)));
-    CK(e, cudaMalloc((void**)&e->d_markq_count, 16));
-    for (auto& ev : e->tev) CK(e, cudaEventCreate(&ev));
-    e->text_on = true;
+    CK(e, dev_alloc(e, tx.tap, S * sizeof(TextTap)));
+    CK(e, cudaMemset(tx.tap, 0, S * sizeof(TextTap)));
+    CK(e, dev_alloc(e, tx.carry, S * cc));
+    CK(e, dev_alloc(e, tx.sparse, 2 * (B + S * cc) + 64));  // per segment: twice its carry and its bytes (content pieces + "error" event texts)
+    CK(e, dev_alloc(e, tx.text, 2 * (B + S * cc) + 64));
+    CK(e, dev_alloc(e, tx.piece_len, (C + 1) * 4));
+    CK(e, dev_alloc(e, tx.seg_len, (S + 1) * 4));
+    CK(e, dev_alloc(e, tx.seg_flags, (S + 1) * 4));
+    CK(e, dev_alloc(e, tx.seg_off, (S + 2) * 8));
+    CK(e, dev_alloc(e, tx.markq, (size_t)(e->lim.rowq_cap + 1) * sizeof(TextMark)));
+    CK(e, dev_alloc(e, tx.markq_count, 16));
+    CK(e, new_events(e, tx.ev, 2));
+    tx.on = true;
     return LGW_OK;
 }
 
 extern "C" int lgw_step_transcript_run(lgw_engine* e, uint64_t* text_bytes, uint32_t* n_marks) {
     if (!e || !text_bytes || !n_marks) return LGW_ERR_ARG;
-    if (!e->text_on) { e->err = "transcripts are not enabled (lgw_transcripts_enable)"; return LGW_ERR_ARG; }
-    if (!e->text_pending) { e->err = "no step to tap (the transcript pass runs once after each lgw_sse_step / lgw_sse_step_device)"; return LGW_ERR_ARG; }
+    lgw_engine::Text& tx = e->text;
+    if (!tx.on) { e->err = "transcripts are not enabled (lgw_transcripts_enable)"; return LGW_ERR_ARG; }
+    if (!tx.pending) { e->err = "no step to tap (the transcript pass runs once after each lgw_sse_step / lgw_sse_step_device)"; return LGW_ERR_ARG; }
     CK(e, cudaSetDevice(e->device));
-    e->text_pending = false;
+    tx.pending = false;
+    const StepArrays& s = e->step.last;
     TextArgs a{};
-    a.data = e->last_bytes; a.chunk_off = e->last_chunk_off; a.seg_chunk = e->last_seg_chunk; a.seg_slot = e->last_seg_slot; a.n_segs = e->last_n_segs;
-    a.seg_res = e->last_seg_out; a.tap = e->d_tap; a.carry = e->d_tcarry; a.carry_cap = e->lim.carry_cap; a.sparse = e->d_tsparse;
-    a.piece_len = e->d_piece_len; a.seg_len = e->d_tseg_len; a.seg_flags = e->d_tseg_flags; a.seg_off = e->d_tseg_off; a.text = e->d_ttext;
-    a.markq = e->d_markq; a.markq_count = e->d_markq_count; a.markq_cap = e->lim.rowq_cap;
-    CK(e, cudaMemsetAsync(e->d_markq_count, 0, 4, e->stream));
-    CK(e, cudaEventRecord(e->tev[0], e->stream));
+    a.data = s.bytes; a.chunk_off = s.chunk_off; a.seg_chunk = s.seg_chunk; a.seg_slot = s.seg_slot; a.n_segs = s.n_segs;
+    a.seg_res = s.seg_out; a.tap = tx.tap; a.carry = tx.carry; a.carry_cap = e->lim.carry_cap; a.sparse = tx.sparse;
+    a.piece_len = tx.piece_len; a.seg_len = tx.seg_len; a.seg_flags = tx.seg_flags; a.seg_off = tx.seg_off; a.text = tx.text;
+    a.markq = tx.markq; a.markq_count = tx.markq_count; a.markq_cap = e->lim.rowq_cap;
+    CK(e, cudaMemsetAsync(tx.markq_count, 0, 4, e->stream));
+    CK(e, cudaEventRecord(tx.ev[0], e->stream));
     const uint32_t n = a.n_segs;
     if (n) {
         k_text_extract<<<(n + TX_WARPS - 1) / TX_WARPS, TX_WARPS * 32, 0, e->stream>>>(a);
         k_text_scan<<<1, 1024, 0, e->stream>>>(a.seg_len, n, a.seg_off);
         k_text_pack<<<(n + TX_WARPS - 1) / TX_WARPS, TX_WARPS * 32, 0, e->stream>>>(a);
         e->launches += 3;
-    } else CK(e, cudaMemsetAsync(e->d_tseg_off, 0, 8, e->stream));
-    CK(e, cudaEventRecord(e->tev[1], e->stream));
+    } else CK(e, cudaMemsetAsync(tx.seg_off, 0, 8, e->stream));
+    CK(e, cudaEventRecord(tx.ev[1], e->stream));
     CK(e, cudaGetLastError());
     unsigned long long total = 0; uint32_t marks = 0;
-    CK(e, cudaMemcpyAsync(&total, e->d_tseg_off + n, 8, cudaMemcpyDeviceToHost, e->stream));
-    CK(e, cudaMemcpyAsync(&marks, e->d_markq_count, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(&total, tx.seg_off + n, 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(&marks, tx.markq_count, 4, cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     if (marks > e->lim.rowq_cap) marks = e->lim.rowq_cap;
-    e->text_total = total; e->text_marks = marks; e->text_ready = true;
-    float t = 0; if (cudaEventElapsedTime(&t, e->tev[0], e->tev[1]) == cudaSuccess) e->tms = t;
+    tx.total = total; tx.marks = marks; tx.ready = true;
+    read_ms(tx.ev[0], tx.ev[1], tx.ms);
     *text_bytes = total; *n_marks = marks;
     return LGW_OK;
 }
 
 extern "C" int lgw_step_transcript_fetch(lgw_engine* e, uint8_t* text_out, uint64_t* seg_text_off, uint32_t* seg_flags, lgw_text_mark* marks_out) {
-    if (!e || !seg_text_off || !seg_flags || (!text_out && e->text_total) || (!marks_out && e->text_marks)) return LGW_ERR_ARG;
-    if (!e->text_ready) { e->err = "lgw_step_transcript_run has not run for the last step"; return LGW_ERR_ARG; }
+    if (!e || !seg_text_off || !seg_flags || (!text_out && e->text.total) || (!marks_out && e->text.marks)) return LGW_ERR_ARG;
+    lgw_engine::Text& tx = e->text;
+    if (!tx.ready) { e->err = "lgw_step_transcript_run has not run for the last step"; return LGW_ERR_ARG; }
     CK(e, cudaSetDevice(e->device));
-    const uint32_t n = e->last_n_segs;
-    if (e->text_total) CK(e, cudaMemcpyAsync(text_out, e->d_ttext, e->text_total, cudaMemcpyDeviceToHost, e->stream));
-    CK(e, cudaMemcpyAsync(seg_text_off, e->d_tseg_off, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, e->stream));
-    if (n) CK(e, cudaMemcpyAsync(seg_flags, e->d_tseg_flags, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
-    if (e->text_marks) CK(e, cudaMemcpyAsync(marks_out, e->d_markq, (size_t)e->text_marks * sizeof(TextMark), cudaMemcpyDeviceToHost, e->stream));
+    const uint32_t n = e->step.last.n_segs;
+    if (tx.total) CK(e, cudaMemcpyAsync(text_out, tx.text, tx.total, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(seg_text_off, tx.seg_off, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, e->stream));
+    if (n) CK(e, cudaMemcpyAsync(seg_flags, tx.seg_flags, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
+    if (tx.marks) CK(e, cudaMemcpyAsync(marks_out, tx.markq, (size_t)tx.marks * sizeof(TextMark), cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     return LGW_OK;
 }
 
 extern "C" int lgw_transcript_last_ms(lgw_engine* e, float* ms) {
     if (!e || !ms) return LGW_ERR_ARG;
-    *ms = e->tms;
+    *ms = e->text.ms;
     return LGW_OK;
 }
 
+// Device memory handed out by lgw_device_alloc is the caller's until lgw_device_free, like the pinned buffers.
 extern "C" int lgw_device_alloc(lgw_engine* e, uint64_t bytes, void** out) {
     if (!e || !out) return LGW_ERR_ARG;
     CK(e, cudaSetDevice(e->device));
@@ -787,15 +846,9 @@ static_assert(sizeof(BodyPlan) == sizeof(lgw_body_plan), "lgw_body_plan");
 static_assert(sizeof(BodyResult) == sizeof(lgw_body_result), "lgw_body_result");
 static_assert(sizeof(BodyScan) == sizeof(lgw_body_scan), "lgw_body_scan");
 
-template <class T>
-static cudaError_t grow(T*& p, uint64_t& cap, uint64_t need) {
-    if (need <= cap && p) return cudaSuccess;
-    if (p) { cudaError_t r = cudaFree(p); p = nullptr; cap = 0; if (r != cudaSuccess) return r; }
-    const uint64_t n = need + need / 4 + 64;
-    cudaError_t r = cudaMalloc((void**)&p, n * sizeof(T));
-    if (r == cudaSuccess) cap = n;
-    return r;
-}
+// Room for n elements in a staging buffer of the body calls.  Batch sizes vary from call to call, so these grow by a quarter
+// and 64 elements beyond the request that outgrew them.
+static cudaError_t reserve_body(DevBuf& b, uint64_t n, size_t elem_size = 1) { return b.reserve(n * elem_size, (n / 4 + 64) * elem_size); }
 
 extern "C" int lgw_rules_load(lgw_engine* e, const lgw_body_plan* plans, uint32_t n_plans,
                               const lgw_body_op* ops, uint32_t n_ops, const uint8_t* blob, uint32_t blob_len) {
@@ -809,34 +862,32 @@ extern "C" int lgw_rules_load(lgw_engine* e, const lgw_body_plan* plans, uint32_
         if ((uint64_t)o.key_off + o.key_len > blob_len || (uint64_t)o.rkey_off + o.rkey_len > blob_len || (uint64_t)o.rval_off + o.rval_len > blob_len) {
             e->err = "lgw_rules_load: op outside the blob"; return LGW_ERR_ARG; }
     }
+    lgw_engine::Bodies& bo = e->bodies;
     CK(e, cudaSetDevice(e->device));
     CK(e, cudaStreamSynchronize(e->stream));
-    cudaFree(e->d_plans); cudaFree(e->d_ops); cudaFree(e->d_blob); e->d_plans = nullptr; e->d_ops = nullptr; e->d_blob = nullptr;
-    CK(e, cudaMalloc((void**)&e->d_plans, (n_plans + 1) * sizeof(BodyPlan)));
-    CK(e, cudaMalloc((void**)&e->d_ops, (n_ops + 1) * sizeof(BodyOp)));
-    CK(e, cudaMalloc((void**)&e->d_blob, blob_len + 16));
-    if (n_plans) CK(e, cudaMemcpyAsync(e->d_plans, plans, n_plans * sizeof(BodyPlan), cudaMemcpyHostToDevice, e->stream));
-    if (n_ops) CK(e, cudaMemcpyAsync(e->d_ops, ops, n_ops * sizeof(BodyOp), cudaMemcpyHostToDevice, e->stream));
-    if (blob_len) CK(e, cudaMemcpyAsync(e->d_blob, blob, blob_len, cudaMemcpyHostToDevice, e->stream));
+    CK(e, bo.plans.reserve((n_plans + 1) * sizeof(BodyPlan)));
+    CK(e, bo.ops.reserve((n_ops + 1) * sizeof(BodyOp)));
+    CK(e, bo.blob.reserve((size_t)blob_len + 16));
+    if (n_plans) CK(e, cudaMemcpyAsync(bo.plans.p, plans, n_plans * sizeof(BodyPlan), cudaMemcpyHostToDevice, e->stream));
+    if (n_ops) CK(e, cudaMemcpyAsync(bo.ops.p, ops, n_ops * sizeof(BodyOp), cudaMemcpyHostToDevice, e->stream));
+    if (blob_len) CK(e, cudaMemcpyAsync(bo.blob.p, blob, blob_len, cudaMemcpyHostToDevice, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
-    e->n_plans = n_plans; e->n_ops = n_ops;
+    bo.n_plans = n_plans; bo.n_ops = n_ops;
     return LGW_OK;
 }
 
 static int bodies_stage_in(lgw_engine* e, const uint8_t* bodies, const uint64_t* body_off, uint32_t n) {
     const uint64_t n_bytes = body_off[n];
     for (uint32_t i = 0; i < n; ++i) if (body_off[i + 1] < body_off[i] || body_off[i + 1] - body_off[i] > 0xFFFFFFF0ull) { e->err = "body offsets not monotonic"; return LGW_ERR_ARG; }
-    CK(e, grow(e->b_in, e->b_in_cap, n_bytes + 64));
-    uint64_t ncap = e->b_n_cap;
-    if (n + 1 > e->b_n_cap || !e->b_off) {
-        uint64_t c1 = e->b_n_cap, c2 = e->b_n_cap, c3 = e->b_n_cap, c4 = e->b_n_cap, c5 = e->b_n_cap;
-        CK(e, grow(e->b_off, c1, n + 1)); CK(e, grow(e->b_out_off, c2, n + 1)); CK(e, grow(e->b_plan_idx, c3, n + 1));
-        CK(e, grow(e->b_results, c4, n + 1)); CK(e, grow(e->b_scans, c5, n + 1));
-        ncap = c1;
-    }
-    e->b_n_cap = ncap;
-    if (n_bytes) CK(e, cudaMemcpyAsync(e->b_in, bodies, n_bytes, cudaMemcpyHostToDevice, e->stream));
-    CK(e, cudaMemcpyAsync(e->b_off, body_off, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
+    lgw_engine::Bodies& bo = e->bodies;
+    CK(e, reserve_body(bo.in, n_bytes + 64));
+    CK(e, reserve_body(bo.off, n + 1, sizeof(uint64_t)));
+    CK(e, reserve_body(bo.out_off, n + 1, sizeof(uint64_t)));
+    CK(e, reserve_body(bo.plan_idx, n + 1, sizeof(uint32_t)));
+    CK(e, reserve_body(bo.results, n + 1, sizeof(BodyResult)));
+    CK(e, reserve_body(bo.scans, n + 1, sizeof(BodyScan)));
+    if (n_bytes) CK(e, cudaMemcpyAsync(bo.in.p, bodies, n_bytes, cudaMemcpyHostToDevice, e->stream));
+    CK(e, cudaMemcpyAsync(bo.off.p, body_off, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
     return LGW_OK;
 }
 
@@ -845,43 +896,45 @@ extern "C" int lgw_bodies_scan(lgw_engine* e, const uint8_t* bodies, const uint6
     if (!e || !body_off || (!bodies && n && body_off[n]) || !scans_out || (model_cap && !models_out)) return LGW_ERR_ARG;
     if (n == 0) return LGW_OK;
     CK(e, cudaSetDevice(e->device));
-    int rc = bodies_stage_in(e, bodies, body_off, n);
-    if (rc != LGW_OK) return rc;
-    CK(e, grow(e->b_models, e->b_models_cap, (uint64_t)n * model_cap + 16));
-    k_body_scan<<<(n + LGW_BODY_WARPS - 1) / LGW_BODY_WARPS, 32 * LGW_BODY_WARPS, 0, e->stream>>>(e->b_in, e->b_off, n, model_cap, e->b_scans, e->b_models);
+    TRY(bodies_stage_in(e, bodies, body_off, n));
+    lgw_engine::Bodies& bo = e->bodies;
+    CK(e, reserve_body(bo.models, (uint64_t)n * model_cap + 16));
+    k_body_scan<<<(n + LGW_BODY_WARPS - 1) / LGW_BODY_WARPS, 32 * LGW_BODY_WARPS, 0, e->stream>>>(bo.in.as<uint8_t>(), bo.off.as<uint64_t>(), n, model_cap, bo.scans.as<BodyScan>(), bo.models.as<uint8_t>());
     ++e->launches;
     CK(e, cudaGetLastError());
-    CK(e, cudaMemcpyAsync(scans_out, e->b_scans, n * sizeof(BodyScan), cudaMemcpyDeviceToHost, e->stream));
-    if (model_cap) CK(e, cudaMemcpyAsync(models_out, e->b_models, (uint64_t)n * model_cap, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(scans_out, bo.scans.p, n * sizeof(BodyScan), cudaMemcpyDeviceToHost, e->stream));
+    if (model_cap) CK(e, cudaMemcpyAsync(models_out, bo.models.p, (uint64_t)n * model_cap, cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     return LGW_OK;
 }
 
 static int bodies_launch(lgw_engine* e, const uint8_t* d_bodies, const uint64_t* d_body_off, uint32_t n, const uint32_t* d_plan_idx,
                          uint32_t slot_cap, uint8_t* d_out, uint64_t out_cap, uint64_t* d_out_off, BodyResult* d_results) {
-    if (!e->d_plans) { e->err = "lgw_bodies_rewrite before lgw_rules_load"; return LGW_ERR_ARG; }
-    CK(e, grow(e->b_slots, e->b_slots_cap, (uint64_t)n * slot_cap + 64));
-    CK(e, grow(e->b_redo, e->b_redo_cap, (uint64_t)n + 4));
-    uint32_t* redo_count = e->b_redo + n;            // list first, counter behind it
-    const uint32_t seq_grid = (n + LGW_BODY_WARPS - 1) / LGW_BODY_WARPS < (uint32_t)e->sm_count * 4u ? (n + LGW_BODY_WARPS - 1) / LGW_BODY_WARPS : (uint32_t)e->sm_count * 4u;
-    CK(e, cudaEventRecord(e->bev[0], e->stream));
-    if (e->body_mode == 0) {
+    lgw_engine::Bodies& bo = e->bodies;
+    if (!bo.plans.p) { e->err = "lgw_bodies_rewrite before lgw_rules_load"; return LGW_ERR_ARG; }
+    CK(e, reserve_body(bo.slots, (uint64_t)n * slot_cap + 64));
+    CK(e, reserve_body(bo.redo, (uint64_t)n + 4, sizeof(uint32_t)));
+    const BodyPlan* d_plans = bo.plans.as<BodyPlan>(); const BodyOp* d_ops = bo.ops.as<BodyOp>(); const uint8_t* d_blob = bo.blob.as<uint8_t>();
+    uint8_t* d_slots = bo.slots.as<uint8_t>();
+    uint32_t* redo = bo.redo.as<uint32_t>(); uint32_t* redo_count = redo + n;            // list first, counter behind it
+    const unsigned seq_grid = grid_for(e, n, LGW_BODY_WARPS, 4);
+    CK(e, cudaEventRecord(bo.ev[0], e->stream));
+    if (bo.mode == 0) {
         CK(e, cudaMemsetAsync(redo_count, 0, 4, e->stream));
-        k_body_fast<<<n, LGW_FAST_THREADS, 0, e->stream>>>(d_bodies, d_body_off, n, d_plan_idx, e->d_plans, e->n_plans, e->d_ops, e->d_blob,
-                                                             e->b_slots, slot_cap, d_results, redo_count, e->b_redo);
-        k_body_rewrite<<<seq_grid, 32 * LGW_BODY_WARPS, 0, e->stream>>>(d_bodies, d_body_off, n, d_plan_idx, e->d_plans, e->n_plans, e->d_ops, e->d_blob,
-                                                                        e->b_slots, slot_cap, d_results, redo_count, e->b_redo);
+        k_body_fast<<<n, LGW_FAST_THREADS, 0, e->stream>>>(d_bodies, d_body_off, n, d_plan_idx, d_plans, bo.n_plans, d_ops, d_blob,
+                                                             d_slots, slot_cap, d_results, redo_count, redo);
+        k_body_rewrite<<<seq_grid, 32 * LGW_BODY_WARPS, 0, e->stream>>>(d_bodies, d_body_off, n, d_plan_idx, d_plans, bo.n_plans, d_ops, d_blob,
+                                                                        d_slots, slot_cap, d_results, redo_count, redo);
         ++e->launches;
     } else {
-        k_body_rewrite<<<seq_grid, 32 * LGW_BODY_WARPS, 0, e->stream>>>(d_bodies, d_body_off, n, d_plan_idx, e->d_plans, e->n_plans, e->d_ops, e->d_blob,
-                                                                        e->b_slots, slot_cap, d_results, nullptr, nullptr);
+        k_body_rewrite<<<seq_grid, 32 * LGW_BODY_WARPS, 0, e->stream>>>(d_bodies, d_body_off, n, d_plan_idx, d_plans, bo.n_plans, d_ops, d_blob,
+                                                                        d_slots, slot_cap, d_results, nullptr, nullptr);
     }
-    CK(e, cudaEventRecord(e->bev[1], e->stream));
+    CK(e, cudaEventRecord(bo.ev[1], e->stream));
     k_body_offsets<<<1, 1024, 0, e->stream>>>(d_results, n, out_cap, d_out_off);
-    CK(e, cudaEventRecord(e->bev[2], e->stream));
-    const uint32_t grid = n < (uint32_t)e->sm_count * 8u ? n : (uint32_t)e->sm_count * 8u;
-    k_body_pack<<<grid, 256, 0, e->stream>>>(e->b_slots, slot_cap, d_results, n, d_out_off, d_out, out_cap);
-    CK(e, cudaEventRecord(e->bev[3], e->stream));
+    CK(e, cudaEventRecord(bo.ev[2], e->stream));
+    k_body_pack<<<grid_for(e, n, 1, 8), 256, 0, e->stream>>>(d_slots, slot_cap, d_results, n, d_out_off, d_out, out_cap);
+    CK(e, cudaEventRecord(bo.ev[3], e->stream));
     e->launches += 3;
     CK(e, cudaGetLastError());
     return LGW_OK;
@@ -903,18 +956,18 @@ extern "C" int lgw_bodies_rewrite(lgw_engine* e, const uint8_t* bodies, const ui
     if (!e || !body_off || (!bodies && n && body_off[n]) || !plan_idx || (!out && out_cap) || !out_off || !results || slot_cap == 0) return LGW_ERR_ARG;
     if (n == 0) { out_off[0] = 0; return LGW_OK; }
     CK(e, cudaSetDevice(e->device));
-    int rc = bodies_stage_in(e, bodies, body_off, n);
-    if (rc != LGW_OK) return rc;
-    CK(e, cudaMemcpyAsync(e->b_plan_idx, plan_idx, n * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
-    CK(e, grow(e->b_out, e->b_out_cap, out_cap + 64));
-    rc = bodies_launch(e, e->b_in, e->b_off, n, e->b_plan_idx, slot_cap, e->b_out, out_cap, e->b_out_off, e->b_results);
-    if (rc != LGW_OK) return rc;
+    TRY(bodies_stage_in(e, bodies, body_off, n));
+    lgw_engine::Bodies& bo = e->bodies;
+    CK(e, cudaMemcpyAsync(bo.plan_idx.p, plan_idx, n * sizeof(uint32_t), cudaMemcpyHostToDevice, e->stream));
+    CK(e, reserve_body(bo.out, out_cap + 64));
+    TRY(bodies_launch(e, bo.in.as<uint8_t>(), bo.off.as<uint64_t>(), n, bo.plan_idx.as<uint32_t>(), slot_cap, bo.out.as<uint8_t>(), out_cap,
+                      bo.out_off.as<uint64_t>(), bo.results.as<BodyResult>()));
     // the packed size is only known on the device: offsets first, then exactly that many bytes
-    CK(e, cudaMemcpyAsync(out_off, e->b_out_off, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
-    CK(e, cudaMemcpyAsync(results, e->b_results, n * sizeof(BodyResult), cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(out_off, bo.out_off.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(results, bo.results.p, n * sizeof(BodyResult), cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     const uint64_t total = out_off[n] < out_cap ? out_off[n] : out_cap;
-    if (total) CK(e, cudaMemcpyAsync(out, e->b_out, total, cudaMemcpyDeviceToHost, e->stream));
+    if (total) CK(e, cudaMemcpyAsync(out, bo.out.p, total, cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     return LGW_OK;
 }
@@ -924,18 +977,14 @@ extern "C" int lgw_documents_usage(lgw_engine* e, const uint8_t* docs, const uin
     if (!e || !doc_off || (!docs && n && doc_off[n]) || (!out && n)) return LGW_ERR_ARG;
     if (n == 0) return LGW_OK;
     CK(e, cudaSetDevice(e->device));
-    int rc = bodies_stage_in(e, docs, doc_off, n);           // (the request-body staging buffers: same layout)
-    if (rc != LGW_OK) return rc;
-    DocUsage* d_out = nullptr;
-    CK(e, cudaMalloc((void**)&d_out, (size_t)n * sizeof(DocUsage)));
-    const uint32_t grid = (n + LGW_DOC_WARPS - 1) / LGW_DOC_WARPS < (uint32_t)e->sm_count * 8u ? (n + LGW_DOC_WARPS - 1) / LGW_DOC_WARPS : (uint32_t)e->sm_count * 8u;
-    k_docs_usage<<<grid, LGW_DOC_WARPS * 32, 0, e->stream>>>(e->b_in, e->b_off, n, d_out);
+    TRY(bodies_stage_in(e, docs, doc_off, n));           // (the request-body staging buffers: same layout)
+    lgw_engine::Bodies& bo = e->bodies;
+    CK(e, bo.doc_out.reserve((size_t)n * sizeof(DocUsage)));
+    k_docs_usage<<<grid_for(e, n, LGW_DOC_WARPS, 8), LGW_DOC_WARPS * 32, 0, e->stream>>>(bo.in.as<uint8_t>(), bo.off.as<uint64_t>(), n, bo.doc_out.as<DocUsage>());
     ++e->launches;
-    cudaError_t r = cudaGetLastError();
-    if (r == cudaSuccess) r = cudaMemcpyAsync(out, d_out, (size_t)n * sizeof(DocUsage), cudaMemcpyDeviceToHost, e->stream);
-    if (r == cudaSuccess) r = cudaStreamSynchronize(e->stream);
-    cudaFree(d_out);
-    if (r != cudaSuccess) { e->err = std::string("lgw_documents_usage: ") + cudaGetErrorString(r); return LGW_ERR_CUDA; }
+    CK(e, cudaGetLastError());
+    CK(e, cudaMemcpyAsync(out, bo.doc_out.p, (size_t)n * sizeof(DocUsage), cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
     return LGW_OK;
 }
 
@@ -944,30 +993,25 @@ extern "C" int lgw_documents_error_detail(lgw_engine* e, const uint8_t* docs, co
     if (!e || !doc_off || (!docs && n && doc_off[n]) || (n && (!out || !text)) || text_stride == 0) return LGW_ERR_ARG;
     if (n == 0) return LGW_OK;
     CK(e, cudaSetDevice(e->device));
-    int rc = bodies_stage_in(e, docs, doc_off, n);
-    if (rc != LGW_OK) return rc;
-    DocError* d_out = nullptr; uint8_t* d_text = nullptr;
-    CK(e, cudaMalloc((void**)&d_out, (size_t)n * sizeof(DocError)));
-    cudaError_t r = cudaMalloc((void**)&d_text, (size_t)n * text_stride);
-    if (r == cudaSuccess) {
-        const uint32_t grid = (n + LGW_DOC_WARPS - 1) / LGW_DOC_WARPS < (uint32_t)e->sm_count * 8u ? (n + LGW_DOC_WARPS - 1) / LGW_DOC_WARPS : (uint32_t)e->sm_count * 8u;
-        k_docs_error_detail<<<grid, LGW_DOC_WARPS * 32, 0, e->stream>>>(e->b_in, e->b_off, n, d_out, d_text, text_stride);
-        ++e->launches;
-        r = cudaGetLastError();
-    }
-    if (r == cudaSuccess) r = cudaMemcpyAsync(out, d_out, (size_t)n * sizeof(DocError), cudaMemcpyDeviceToHost, e->stream);
-    if (r == cudaSuccess) r = cudaMemcpyAsync(text, d_text, (size_t)n * text_stride, cudaMemcpyDeviceToHost, e->stream);
-    if (r == cudaSuccess) r = cudaStreamSynchronize(e->stream);
-    cudaFree(d_out); cudaFree(d_text);
-    if (r != cudaSuccess) { e->err = std::string("lgw_documents_error_detail: ") + cudaGetErrorString(r); return LGW_ERR_CUDA; }
+    TRY(bodies_stage_in(e, docs, doc_off, n));
+    lgw_engine::Bodies& bo = e->bodies;
+    CK(e, bo.doc_out.reserve((size_t)n * sizeof(DocError)));
+    CK(e, bo.doc_text.reserve((size_t)n * text_stride));
+    k_docs_error_detail<<<grid_for(e, n, LGW_DOC_WARPS, 8), LGW_DOC_WARPS * 32, 0, e->stream>>>(bo.in.as<uint8_t>(), bo.off.as<uint64_t>(), n, bo.doc_out.as<DocError>(), bo.doc_text.as<uint8_t>(), text_stride);
+    ++e->launches;
+    CK(e, cudaGetLastError());
+    CK(e, cudaMemcpyAsync(out, bo.doc_out.p, (size_t)n * sizeof(DocError), cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(text, bo.doc_text.p, (size_t)n * text_stride, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
     return LGW_OK;
 }
 
 extern "C" int lgw_bodies_last_ms(lgw_engine* e, float ms[3]) {
     if (!e || !ms) return LGW_ERR_ARG;
     CK(e, cudaSetDevice(e->device));
-    cudaEventSynchronize(e->bev[3]);
-    for (int i = 0; i < 3; ++i) { float t = 0; if (cudaEventElapsedTime(&t, e->bev[i], e->bev[i + 1]) == cudaSuccess) e->bms[i] = t; ms[i] = e->bms[i]; }
+    lgw_engine::Bodies& bo = e->bodies;
+    cudaEventSynchronize(bo.ev[3]);
+    for (int i = 0; i < 3; ++i) { read_ms(bo.ev[i], bo.ev[i + 1], bo.ms[i]); ms[i] = bo.ms[i]; }
     return LGW_OK;
 }
 

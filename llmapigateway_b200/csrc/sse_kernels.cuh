@@ -68,23 +68,20 @@ __global__ void __launch_bounds__(256) k_copy(const uint8_t* __restrict__ in, ui
 
 #include "relay2.cuh"
 
-static inline cudaError_t scratch_alloc(StepScratch& s, size_t max_streams, size_t max_bytes, int sm_count) {
+// The step's scratch.  alloc(pointer, bytes) -> cudaError_t is the caller's allocator: the memory is the caller's to release.
+template <class Alloc>
+static inline cudaError_t scratch_alloc(StepScratch& s, size_t max_streams, size_t max_bytes, Alloc alloc) {
     cudaError_t r;
-    if ((r = cudaMalloc((void**)&s.plan, max_streams * sizeof(SegPlan))) != cudaSuccess) return r;
-    if ((r = cudaMalloc((void**)&s.tpl_cache2, sizeof(TemplateCache2))) != cudaSuccess) return r;
+    if ((r = alloc(s.plan, max_streams * sizeof(SegPlan))) != cudaSuccess) return r;
+    if ((r = alloc(s.tpl_cache2, sizeof(TemplateCache2))) != cudaSuccess) return r;
     if ((r = cudaMemset(s.tpl_cache2, 0, sizeof(TemplateCache2))) != cudaSuccess) return r;
-    (void)sm_count;
-    if ((r = cudaMalloc((void**)&s.usage_fields, max_streams * 9 * sizeof(uint2))) != cudaSuccess) return r;
-    if ((r = cudaMalloc((void**)&s.tile_seg, (max_bytes / R2_TILE + 4) * 4)) != cudaSuccess) return r;
+    if ((r = alloc(s.usage_fields, max_streams * 9 * sizeof(uint2))) != cudaSuccess) return r;
+    if ((r = alloc(s.tile_seg, (max_bytes / R2_TILE + 4) * 4)) != cudaSuccess) return r;
     if ((r = cudaMemset(s.tile_seg, 0, (max_bytes / R2_TILE + 4) * 4)) != cudaSuccess) return r;
-    if ((r = cudaMalloc((void**)&s.counters, 64)) != cudaSuccess) return r;
+    if ((r = alloc(s.counters, 64)) != cudaSuccess) return r;
     if ((r = cudaMemset(s.counters, 0, 64)) != cudaSuccess) return r;
     if ((r = cudaFuncSetAttribute(k_relay2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)R2_SMEM_BYTES)) != cudaSuccess) return r;
     return cudaSuccess;
-}
-static inline void scratch_free(StepScratch& s) {
-    cudaFree(s.plan); cudaFree(s.tpl_cache2); cudaFree(s.usage_fields); cudaFree(s.counters); s.counters = nullptr; cudaFree(s.tile_seg); s.tile_seg = nullptr;
-    s.plan = nullptr; s.tpl_cache2 = nullptr; s.usage_fields = nullptr;
 }
 
 // Launch one step on `stream`.  ev[0..3] bracket prime / relay / commit (ev[4] = ev[3]: usage extraction is inside relay and commit).

@@ -82,7 +82,8 @@ class Engine:
             pass
 
     def alloc_pinned(self, nbytes: int) -> np.ndarray:
-        """Page-locked host memory owned by the engine (lgw_alloc_pinned) as a uint8 array; freed with the engine."""
+        """Page-locked host memory (lgw_alloc_pinned) as a uint8 array.  The engine keeps no record of it and closing the
+        engine does not free it: it is the caller's until lgw_free_pinned, so arrays that view it stay valid."""
         p = C.c_void_p()
         self._ck(self._lib.lgw_alloc_pinned(self._h, nbytes, C.byref(p)), "alloc_pinned")
         return np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(p.value))
