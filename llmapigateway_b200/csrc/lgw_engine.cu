@@ -696,7 +696,7 @@ extern "C" int lgw_usage_latest(lgw_engine* e, const int64_t* d_ts_us, uint64_t 
     }
     k_list_tile_count<<<ctiles, 1024, 0, e->stream>>>(d_ts_us, N, sel, scan);
     k_list_scan<<<1, 1024, 0, e->stream>>>(scan, ctiles, selected);
-    k_list_tile_write<<<ctiles, 1024, 0, e->stream>>>(d_ts_us, N, sel, scan, keys[0], idx[0]);
+    k_list_tile_write<<<ctiles, 1024, 0, e->stream>>>(d_ts_us, N, sel, scan, M, keys[0], idx[0]);
     e->launches += 1 + 3 * LGW_LIST_DIGITS - 1 + 3;
     if (M <= LGW_LIST_SMEM_SORT) {
         uint32_t p = 1;

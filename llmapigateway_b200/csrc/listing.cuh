@@ -209,9 +209,11 @@ __global__ void __launch_bounds__(1024) k_list_scan(uint32_t* v, uint32_t len, u
     if (threadIdx.x == 0) totals[blockIdx.x] = base;
 }
 
-// the keys between the two boundaries, in index order, at the tile offsets k_list_scan made
+// the keys between the two boundaries, in index order, at the tile offsets k_list_scan made.  Only the first `count` are stored:
+// keys / idx hold `count` entries, and a selection that put more records between the boundaries is caught by the host's check
+// of the total (k_list_scan's), not by writing past them into the rest of the scratch.
 __global__ void __launch_bounds__(1024) k_list_tile_write(const int64_t* __restrict__ ts, uint32_t n, const ListSel* __restrict__ sp, const uint32_t* __restrict__ tile_off,
-                                                          uint64_t* __restrict__ keys, uint32_t* __restrict__ idx) {
+                                                          uint32_t count, uint64_t* __restrict__ keys, uint32_t* __restrict__ idx) {
     __shared__ uint32_t warp_sums[32];
     const ListSel s = *sp;
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -225,8 +227,8 @@ __global__ void __launch_bounds__(1024) k_list_tile_write(const int64_t* __restr
     __syncthreads();
     uint32_t pos = tile_off[blockIdx.x] + __popc(ma & lt) + __popc(mb & lt);
     for (uint32_t w = 0; w < warp; ++w) pos += warp_sums[w];
-    if (ia) { keys[pos] = ka; idx[pos] = 2 * j; ++pos; }
-    if (ib) { keys[pos] = kb; idx[pos] = 2 * j + 1; }
+    if (ia) { if (pos < count) { keys[pos] = ka; idx[pos] = 2 * j; } ++pos; }
+    if (ib && pos < count) { keys[pos] = kb; idx[pos] = 2 * j + 1; }
 }
 
 // pages up to LGW_LIST_SMEM_SORT: bitonic sort of (kd, index) in shared memory by one block; indices out as uint64
