@@ -365,7 +365,8 @@ enum lgw_text_flag {
     LGW_TF_EXOTIC = 1 << 1,          /* an event shape whose Python behaviour the device does not model: text not authoritative */
     LGW_TF_CARRY_OVERFLOW = 1 << 2,  /* an unterminated event outgrew carry_cap */
     LGW_TF_MARKQ_OVERFLOW = 1 << 3,  /* more marks in one step than rowq_cap */
-    LGW_TF_SEQUENTIAL = 1 << 4       /* (this step) the segment took the sequential walk */
+    LGW_TF_SEQUENTIAL = 1 << 4,      /* (this step) the segment took the sequential walk */
+    LGW_TF_DOC_ERROR_LOG = 1 << 5    /* (lgw_documents_text) the document has a top-level "error": write_log ran at :139 too */
 };
 typedef struct lgw_text_mark { uint32_t slot, seq; uint64_t text_pos; } lgw_text_mark;
 int lgw_transcripts_enable(lgw_engine* e);
@@ -374,6 +375,17 @@ int lgw_step_transcript_fetch(lgw_engine* e, uint8_t* text_out /* text_bytes */,
                               uint32_t* seg_flags /* n_segs */, lgw_text_mark* marks_out /* n_marks */);
 /* device time of the last transcript pass (extract + scan + pack), milliseconds */
 int lgw_transcript_last_ms(lgw_engine* e, float* ms);
+
+/* text the non-streaming tap accumulates for each document (chat_logging.py:97-150, the documents of lgw_documents_usage): the whole
+ * document is one part; for every choice `delta.content` else `message.content` when truthy, JSON escapes decoded, plus the document's
+ * own text when it has a top-level "error".  Text of doc i = text_out[text_off[i] .. text_off[i+1]) (UTF-8, a lone surrogate in
+ * 'surrogatepass' form); flags[i]: LGW_TF_LONE_SURROGATE / LGW_TF_EXOTIC, and LGW_TF_DOC_ERROR_LOG when write_log ran at :139 as
+ * well as at :150 (both calls write this text).  A text_cap of twice the batch's bytes always suffices; when the text does not fit
+ * the call returns LGW_ERR_CAPACITY before anything is copied out.  Documents are limited to 2^31 bytes. */
+int lgw_documents_text(lgw_engine* e, const uint8_t* docs, const uint64_t* doc_off /* n+1 */, uint32_t n,
+                       uint8_t* text_out, uint64_t text_cap, uint64_t* text_off /* n+1 */, uint32_t* flags /* n */);
+/* device time of the last lgw_documents_text (walk + scan + pack), milliseconds */
+int lgw_documents_text_last_ms(lgw_engine* e, float* ms);
 
 /* ---- device memory helpers for callers without their own CUDA allocator ----------------------------- */
 int lgw_device_alloc(lgw_engine* e, uint64_t bytes, void** out);

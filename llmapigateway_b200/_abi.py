@@ -47,6 +47,7 @@ class TextMark(C.Structure):
 
 
 TF_LONE_SURROGATE, TF_EXOTIC, TF_CARRY_OVERFLOW, TF_MARKQ_OVERFLOW, TF_SEQUENTIAL = 1, 2, 4, 8, 16
+TF_DOC_ERROR_LOG = 32          # lgw_documents_text: the document's top-level "error" made write_log run at chat_logging.py:139 too
 
 
 class SegResult(C.Structure):

@@ -22,6 +22,7 @@ EXPORTS = [
     "lgw_device_alloc", "lgw_device_free", "lgw_device_upload", "lgw_device_download", "lgw_device_zero",
     "lgw_transcripts_enable", "lgw_step_transcript_run", "lgw_step_transcript_fetch", "lgw_transcript_last_ms",
     "lgw_documents_usage", "lgw_rules_load", "lgw_bodies_scan", "lgw_bodies_rewrite", "lgw_bodies_rewrite_device", "lgw_bodies_last_ms",
+    "lgw_documents_text", "lgw_documents_text_last_ms",
 ]
 
 _lib = None
@@ -93,6 +94,8 @@ def load():
     lib.lgw_step_transcript_run.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
     lib.lgw_step_transcript_fetch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.lgw_transcript_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
+    lib.lgw_documents_text.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
+    lib.lgw_documents_text_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
     if hasattr(lib, "lgw_engine_set_mode"):
         lib.lgw_engine_set_mode.argtypes = [C.c_void_p, C.c_int]
     if lib.lgw_abi_version() != 1:

@@ -3,10 +3,12 @@
 // One warp per document: the lanes stage the text in shared memory, one lane runs the full machine (json_machine.cuh) over
 // it -- the same machine and the same tap rules (tap_part, stream_machine.cuh) as the streaming path, so the two modes cannot
 // drift apart.  Documents longer than the stage are read from global memory.
+// k_docs_text reads out the text the same tap accumulates (transcript.cuh doc_text) for the log files of chat transcripts.
 #pragma once
 #include <cuda_runtime.h>
 #include "stream_machine.cuh"
 #include "error_detail.cuh"
+#include "transcript.cuh"
 
 namespace lgw {
 
@@ -67,6 +69,45 @@ __global__ void __launch_bounds__(LGW_DOC_WARPS * 32) k_docs_error_detail(const 
         __syncwarp();
         if (lane == 0) error_detail_of(staged ? stage[warp] : src, len, out[i], text + (size_t)i * text_stride, text_stride);
         __syncwarp();
+    }
+}
+
+// text the tap accumulates for each non-streaming response (chat_logging.py:124-139, transcript.cuh doc_text), in k_docs_usage's
+// geometry.  Document i writes its text to the sparse buffer at 2 * (off[i] - off[0]) (room: twice its length), its length to len[i]
+// and its TextFlag bits to flags[i].  k_text_scan turns the lengths into offsets and k_docs_text_pack packs the pieces.
+__global__ void __launch_bounds__(LGW_DOC_WARPS * 32) k_docs_text(const uint8_t* __restrict__ docs, const uint64_t* __restrict__ off, uint32_t n,
+                                                                  uint8_t* __restrict__ sparse, uint32_t* __restrict__ len_out, uint32_t* __restrict__ flags_out) {
+    __shared__ __align__(16) uint8_t stage[LGW_DOC_WARPS][LGW_DOC_STAGE];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+    const uint64_t base = off[0];
+    for (uint32_t i = blockIdx.x * LGW_DOC_WARPS + warp; i < n; i += gridDim.x * LGW_DOC_WARPS) {
+        const uint8_t* src = docs + off[i];
+        const uint32_t len = (uint32_t)(off[i + 1] - off[i]);              // (the engine limits documents to 2^31 bytes: 2 * len fits)
+        const bool staged = len <= LGW_DOC_STAGE;
+        if (staged) for (uint32_t k = lane; k < len; k += 32) stage[warp][k] = src[k];
+        __syncwarp();
+        if (lane == 0) {
+            Rope r{nullptr, 0, staged ? stage[warp] : src, len};
+            TextOut o{sparse + 2 * (off[i] - base), 0, 0};
+            const bool logged = doc_text(r, len, o);
+            len_out[i] = o.pos;
+            flags_out[i] = o.flags | (logged ? (uint32_t)TF_DOC_ERROR_LOG : 0u);
+        }
+        __syncwarp();
+    }
+}
+
+// the pieces of k_docs_text, document after document: text[text_off[i] ..) = sparse[2 * (off[i] - off[0]) ..), one warp per document
+__global__ void __launch_bounds__(LGW_DOC_WARPS * 32) k_docs_text_pack(const uint64_t* __restrict__ off, uint32_t n, const uint8_t* __restrict__ sparse,
+                                                                       const uint32_t* __restrict__ len, const unsigned long long* __restrict__ text_off,
+                                                                       uint8_t* __restrict__ text) {
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+    const uint64_t base = off[0];
+    for (uint32_t i = blockIdx.x * LGW_DOC_WARPS + warp; i < n; i += gridDim.x * LGW_DOC_WARPS) {
+        const uint8_t* src = sparse + 2 * (off[i] - base);
+        uint8_t* dst = text + text_off[i];
+        const uint32_t m = len[i];
+        for (uint32_t k = lane; k < m; k += 32) dst[k] = src[k];
     }
 }
 

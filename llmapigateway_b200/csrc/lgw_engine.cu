@@ -110,6 +110,10 @@ struct lgw_engine {
         int mode = 0;               // 0: data-parallel path + exact machine for the rest, 1: exact machine only (tests)
         cudaEvent_t ev[4]{}; float ms[3]{0, 0, 0};
     } bodies;
+    struct DocsText {               // lgw_documents_text (doc_kernels.cuh): input in the body staging, events created on first use
+        DevBuf sparse, len, flags, off, text;
+        cudaEvent_t ev[2]{}; float ms = 0;
+    } docs_text;
     struct Text {                   // transcript tap (transcript.cuh; off until lgw_transcripts_enable)
         bool on = false, pending = false, ready = false;
         TextTap* tap = nullptr; uint8_t *carry = nullptr, *sparse = nullptr, *text = nullptr;
@@ -1003,6 +1007,50 @@ extern "C" int lgw_documents_error_detail(lgw_engine* e, const uint8_t* docs, co
     CK(e, cudaMemcpyAsync(out, bo.doc_out.p, (size_t)n * sizeof(DocError), cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaMemcpyAsync(text, bo.doc_text.p, (size_t)n * text_stride, cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
+    return LGW_OK;
+}
+
+// ---- text of the non-streaming tap (row a8, chat_logging.py:124-139): walk, scan of the lengths, pack -----------------------
+extern "C" int lgw_documents_text(lgw_engine* e, const uint8_t* docs, const uint64_t* doc_off, uint32_t n,
+                                  uint8_t* text_out, uint64_t text_cap, uint64_t* text_off, uint32_t* flags) {
+    if (!e || !doc_off || (!docs && n && doc_off[n]) || !text_off || (!flags && n) || (!text_out && text_cap)) return LGW_ERR_ARG;
+    if (n == 0) { text_off[0] = 0; return LGW_OK; }
+    for (uint32_t i = 0; i < n; ++i)
+        if (doc_off[i + 1] >= doc_off[i] && doc_off[i + 1] - doc_off[i] > 0x7FFFFFFFull) { e->err = "document longer than 2^31 bytes"; return LGW_ERR_ARG; }
+    CK(e, cudaSetDevice(e->device));
+    TRY(bodies_stage_in(e, docs, doc_off, n));           // (the request-body staging buffers: same layout)
+    lgw_engine::DocsText& dt = e->docs_text;
+    if (!dt.ev[0]) CK(e, new_events(e, dt.ev, 2));
+    const uint64_t room = 2 * (doc_off[n] - doc_off[0]);  // a document's text is at most twice its length (transcript.cuh text_part)
+    CK(e, reserve_body(dt.sparse, room + 64));
+    CK(e, reserve_body(dt.text, room + 64));
+    CK(e, reserve_body(dt.len, n + 1, sizeof(uint32_t)));
+    CK(e, reserve_body(dt.flags, n + 1, sizeof(uint32_t)));
+    CK(e, reserve_body(dt.off, n + 1, sizeof(unsigned long long)));
+    const uint64_t* d_off = e->bodies.off.as<uint64_t>();
+    const unsigned grid = grid_for(e, n, LGW_DOC_WARPS, 8);
+    CK(e, cudaEventRecord(dt.ev[0], e->stream));
+    k_docs_text<<<grid, LGW_DOC_WARPS * 32, 0, e->stream>>>(e->bodies.in.as<uint8_t>(), d_off, n, dt.sparse.as<uint8_t>(), dt.len.as<uint32_t>(), dt.flags.as<uint32_t>());
+    k_text_scan<<<1, 1024, 0, e->stream>>>(dt.len.as<uint32_t>(), n, dt.off.as<unsigned long long>());
+    k_docs_text_pack<<<grid, LGW_DOC_WARPS * 32, 0, e->stream>>>(d_off, n, dt.sparse.as<uint8_t>(), dt.len.as<uint32_t>(), dt.off.as<unsigned long long>(), dt.text.as<uint8_t>());
+    CK(e, cudaEventRecord(dt.ev[1], e->stream));
+    e->launches += 3;
+    CK(e, cudaGetLastError());
+    unsigned long long total = 0;
+    CK(e, cudaMemcpyAsync(&total, dt.off.as<unsigned long long>() + n, 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    read_ms(dt.ev[0], dt.ev[1], dt.ms);
+    if (total > text_cap) { e->err = "lgw_documents_text: text_cap is smaller than the text (" + std::to_string(total) + " bytes)"; return LGW_ERR_CAPACITY; }
+    if (total) CK(e, cudaMemcpyAsync(text_out, dt.text.p, total, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(text_off, dt.off.p, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(flags, dt.flags.p, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    return LGW_OK;
+}
+
+extern "C" int lgw_documents_text_last_ms(lgw_engine* e, float* ms) {
+    if (!e || !ms) return LGW_ERR_ARG;
+    *ms = e->docs_text.ms;
     return LGW_OK;
 }
 

@@ -31,7 +31,8 @@ enum TextFlag : uint32_t {
     TF_EXOTIC = 1u << 1,           // an event had a shape whose Python behaviour the device does not model: the text is not authoritative
     TF_CARRY_OVERFLOW = 1u << 2,   // an unterminated event outgrew carry_cap (engine limit)
     TF_MARKQ_OVERFLOW = 1u << 3,
-    TF_SEQUENTIAL = 1u << 4        // (per step) the segment took the sequential walk
+    TF_SEQUENTIAL = 1u << 4,       // (per step) the segment took the sequential walk
+    TF_DOC_ERROR_LOG = 1u << 5     // (per document, doc_text) the document made the tap call write_log at chat_logging.py:139
 };
 
 struct TextTap {               // per-stream state of the transcript tap
@@ -116,6 +117,15 @@ LGW_HD_NOINLINE bool text_part(const Rope& r, uint32_t s, uint32_t e, uint8_t cl
     if (cls == PC_DATA) while (te > t0 && JsonMachine<false>::is_py_ws(r.at(te - 1))) --te;
     for (uint32_t i = t0; i < te; ++i) o.p[o.pos++] = (uint8_t)r.at(i);               // :138 accum += decoded_chunk
     return true;
+}
+
+// The tap of a non-streaming response (chat_logging.py:97-150 with is_real_streaming=False): the joined chunks are ONE part
+// (:105-106), walked by the per-part code above.  Appends the document's llm_response_accum to `o` (room: twice the document);
+// returns true when the tap calls write_log at :139 as well as at :150.  Both calls write the same text.
+LGW_HD bool doc_text(const Rope& r, uint32_t len, TextOut& o) {
+    const uint8_t cls = classify_part(r, 0, len);                                       // :116-121
+    if (cls == PC_NONE) return false;
+    return text_part(r, 0, len, cls, o, true);
 }
 
 struct TextIO {

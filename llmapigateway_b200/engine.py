@@ -303,6 +303,25 @@ class Engine:
             res.append(([dict(row), row] if out[i].error_row else [row], bool(out[i].exotic)))
         return res
 
+    def documents_text(self, docs):
+        """The text the same tap accumulates for every document (chat_logging.py:124-139): what both of its write_log calls write.
+        -> list of (text bytes: UTF-8, a lone surrogate in 'surrogatepass' form; flags: _abi.TF_* bits, TF_DOC_ERROR_LOG when the
+        document has the extra row of documents_usage)"""
+        from . import rewrite as rw
+        buf, off = rw.pack_bodies(docs)
+        n = len(docs)
+        text = np.empty(max(2 * int(off[n] - off[0]), 1), dtype=np.uint8)
+        text_off = np.zeros(n + 1, dtype=np.uint64)
+        flags = np.zeros(max(n, 1), dtype=np.uint32)
+        self._ck(self._lib.lgw_documents_text(self._h, _ptr(buf), _ptr(off), n, _ptr(text), text.size, _ptr(text_off), _ptr(flags)),
+                 "documents_text")
+        return [(text[int(text_off[i]):int(text_off[i + 1])].tobytes(), int(flags[i])) for i in range(n)]
+
+    def documents_text_last_ms(self) -> float:
+        ms = C.c_float(0)
+        self._ck(self._lib.lgw_documents_text_last_ms(self._h, C.byref(ms)), "documents_text_last_ms")
+        return ms.value
+
     def documents_error_detail(self, docs, text_stride: int = 4096):
         """request_handler.py:167-169 for failing non-streaming responses -> list of (DocError, text bytes)."""
         from . import rewrite as rw

@@ -186,6 +186,13 @@ class StreamBatcher:
         """Response tap of non-streaming responses (chat_logging.py:98-150): the usage rows of each document."""
         return await asyncio.get_running_loop().run_in_executor(self._worker, self.eng.documents_usage, list(docs))
 
+    async def documents_tap(self, docs):
+        """The whole non-streaming tap of each document, in one worker call: [((rows, exotic), (text, text flags))] -- the rows
+        of documents_usage and the text every one of those write_log calls writes (Engine.documents_text)."""
+        def _both(docs):
+            return list(zip(self.eng.documents_usage(docs), self.eng.documents_text(docs)))
+        return await asyncio.get_running_loop().run_in_executor(self._worker, _both, list(docs))
+
     async def detail(self, slot: int) -> str:
         raw = await asyncio.get_running_loop().run_in_executor(self._worker, self.eng.detail, slot)
         return raw.decode("utf-8", errors="replace")
@@ -404,9 +411,19 @@ async def log_chat_completions(request, call_next, *, batcher: StreamBatcher):
     /chat/completions route -- non-streaming completions, and the 400/503 JSON bodies of the endpoint -- is what the reference
     hands to a ChunkProcessorThread in its non-streaming mode (:188-190, :98-150): the body is collected, the engine reads the
     usage row(s) out of it (lgw_documents_usage) and they go to the usage sink; the client gets the same bytes, re-chunked
-    exactly as they came."""
+    exactly as they came.  When the batcher keeps transcripts (a `TranscriptLog`), the request is read first as the reference
+    reads it (:170-178) and every row goes through write_log with the document's text (lgw_documents_text): the log file, then the
+    row."""
     if not request.url.path.endswith("/chat/completions"):               # :167-168
         return await call_next(request)
+    req = None
+    if getattr(batcher, "transcript_log", None) is not None:
+        try:                                                              # :170-178 (any failure: the response goes out untapped)
+            req_body_bytes = await request.body()
+            req_body_str = req_body_bytes.decode("utf-8") if req_body_bytes else ""
+            req = (dict(request.headers), req_body_str)
+        except Exception:
+            return await call_next(request)
     response = await call_next(request)
     try:
         if getattr(response, "lgw_tapped", False):
@@ -422,11 +439,17 @@ async def log_chat_completions(request, call_next, *, batcher: StreamBatcher):
                 async for chunk in original:
                     chunks.append(bytes(chunk))
                     yield chunk
-                await _tap_document(batcher, chunks)
+                if req is None:
+                    await _tap_document(batcher, chunks)
+                else:
+                    await _tap_document_logged(batcher, chunks, req)
 
             response.body_iterator = tapping()
         elif getattr(response, "body", None) is not None:
-            await _tap_document(batcher, [bytes(response.body)])
+            if req is None:
+                await _tap_document(batcher, [bytes(response.body)])
+            else:
+                await _tap_document_logged(batcher, [bytes(response.body)], req)
     except Exception:                                                     # :228-229 the middleware never breaks the response
         pass
     return response
@@ -443,6 +466,22 @@ async def _tap_document(batcher: StreamBatcher, chunks):
     rows, _exotic = (await batcher.documents_usage([text]))[0]
     for row in rows:
         batcher._sink(row)
+
+
+async def _tap_document_logged(batcher: StreamBatcher, chunks, req):
+    """_tap_document with transcripts: every write_log call of the tap (:139 for a top-level "error", then :150) writes the log
+    file with the document's text and then inserts its row; a text the file cannot hold (a lone surrogate) gives neither."""
+    if not chunks:                                                        # no first chunk => no thread => no file, no row
+        return
+    try:
+        text = b"".join(chunks)
+        text.decode("utf-8")                                              # (:101)
+    except UnicodeDecodeError:
+        return
+    (rows, _exotic), (accum, _tflags) = (await batcher.documents_tap([text]))[0]
+    req_headers, req_body_str = req
+    for row in rows:
+        batcher.transcript_log.write_log(req_headers, req_body_str, accum, row)
 
 
 class SqliteUsageSink:
