@@ -22,6 +22,7 @@ import numpy as np
 
 from . import _abi
 from . import rewrite as rw
+from .details import attempt_detail
 from .gateway import StreamBatcher, make_llm_request, shard_of
 
 
@@ -496,6 +497,7 @@ class ChainBatch:
                 out.steps += 1
                 out.round_out[-1] = r.out
                 phase, verdict, eb = r.segs["phase"], r.segs["verdict"], r.segs["emit_chunk_begin"].astype(np.int64)
+                sflags = r.segs["flags"]
                 is_failed = phase == _abi.PHASE_FAILED
                 fidx = np.nonzero(is_failed)[0]
                 dets = eng.details(slots[fidx])
@@ -504,6 +506,10 @@ class ChainBatch:
                     i = int(sreq[k])
                     if verdict[k] == _abi.VERDICT_FAIL_PARSE:
                         d = f"Unexpected error during request to {sched_list[sid[i]][rnd][1]}: first event is not valid JSON: {d.decode('utf-8', errors='replace')[:200]}"
+                    elif sflags[k] & _abi.SF_DETAIL_TRUNC:                       # longer than detail_cap: the whole event from the answer
+                        co = ans.chunk_off
+                        d = attempt_detail(d, int(verdict[k]), int(sflags[k]),
+                                           [ans.data[int(co[c]):int(co[c + 1])] for c in range(int(ans.seg_chunk[k]), int(ans.seg_chunk[k + 1]))])
                     fail_text[i] = d
                 fail_round[sreq[fidx]] = rnd
                 failed_now.append(sreq[fidx])

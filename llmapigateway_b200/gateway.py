@@ -21,6 +21,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from . import _abi
+from .details import attempt_detail
 
 
 def shard_of(stream_id, n_gpus: int) -> int:
@@ -193,9 +194,9 @@ class StreamBatcher:
             return list(zip(self.eng.documents_usage(docs), self.eng.documents_text(docs)))
         return await asyncio.get_running_loop().run_in_executor(self._worker, _both, list(docs))
 
-    async def detail(self, slot: int) -> str:
-        raw = await asyncio.get_running_loop().run_in_executor(self._worker, self.eng.detail, slot)
-        return raw.decode("utf-8", errors="replace")
+    async def detail_bytes(self, slot: int) -> bytes:
+        """The engine's copy of a failed attempt's first event: at most detail_cap bytes (details.attempt_detail gives the text)."""
+        return await asyncio.get_running_loop().run_in_executor(self._worker, self.eng.detail, slot)
 
     # -- data ------------------------------------------------------------------------------------------
     async def feed(self, slot: int, chunk: bytes) -> FeedResult:
@@ -363,11 +364,14 @@ async def make_llm_request(target_url: str, headers: dict, payload: dict, is_str
         slot = await batcher.open_stream(response.status_code, **(log_request or {}))
         chunks = response.aiter_bytes()
         first_kept: list[bytes] = []
+        primed: list[bytes] = []          # every chunk fed while priming: the whole first event when the engine's detail is cut
         committed = False
         async for chunk in chunks:                                        # priming: request_handler.py:69-95
+            primed.append(chunk)
             r = await batcher.feed(slot, chunk)
             if r.phase == _abi.PHASE_FAILED:
-                detail = await batcher.detail(slot)
+                raw = await batcher.detail_bytes(slot)
+                detail = attempt_detail(raw, r.verdict, r.flags, primed)
                 if r.verdict == _abi.VERDICT_FAIL_PARSE:                  # :183-187 (message tail is the JSON library's text: unpinned)
                     detail = f"Unexpected error during request to {target_url}: first event is not valid JSON: {detail[:200]}"
                 await _release()
