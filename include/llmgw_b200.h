@@ -251,6 +251,18 @@ int lgw_usage_latest(lgw_engine* e, const int64_t* d_ts_us, uint64_t n, uint64_t
 /* device time of the last lgw_usage_latest, milliseconds (0 after a call with count == 0) */
 int lgw_usage_latest_last_ms(lgw_engine* e, float* ms);
 
+/* cleanup_old_records (tokens_usage_db.py:164-198, `DELETE FROM tokens_usage WHERE timestamp < ?`): the n device-resident
+ * records whose ts_us >= cutoff_us, written in index order (a stable compaction) into the fresh columns d_out.  d_in / d_out
+ * hold the eight column pointers in UsageTable.COLS order: ts_us (int64), model_rank, prompt, completion, total, reasoning,
+ * cached (int32), cost (double); d_out has room for n_keep records per column and must not overlap d_in.  n_keep is the survivor
+ * count the caller computed; only places below it are written, and a device count that differs fails the call (LGW_ERR_CUDA,
+ * message in lgw_last_error) with nothing written past the output.  n >= 2^32, n_keep > n, a null pointer when n > 0 (d_out
+ * may be null when n_keep == 0) or a d_in[0] that is not 16-byte aligned: LGW_ERR_ARG.  n == 0 launches nothing.
+ * Device work: k_retain_count, k_list_scan, k_retain_write (csrc/retain.cuh). */
+int lgw_usage_retain(lgw_engine* e, void* const d_in[8], void* const d_out[8], uint64_t n, int64_t cutoff_us, uint64_t n_keep);
+/* device time of the last lgw_usage_retain, milliseconds (0 after a call with n == 0) */
+int lgw_usage_retain_last_ms(lgw_engine* e, float* ms);
+
 /* ---- request-body rewrite: SURVEY 8 rows a1, a3, a4 --------------------------------------------------
  * Replaces, for a batch of client requests, chat.py:31-45 (parse: lgw_bodies_scan) and, per upstream
  * attempt, chat.py:112-119,:135-139,:150,:164-168 (deepcopy + key assignments) followed by the encoder

@@ -11,6 +11,7 @@
 #include "sse_kernels.cuh"
 #include "rollup.cuh"
 #include "listing.cuh"
+#include "retain.cuh"
 #include "body_kernels.cuh"
 #include "doc_kernels.cuh"
 #include "transcript.cuh"
@@ -102,6 +103,10 @@ struct lgw_engine {
         DevBuf buf; bool attr_set = false;
         cudaEvent_t ev[2]{}; float ms = 0;
     } listing;
+    struct Retain {                 // deleting old records (retain.cuh): tile counts / offsets and the total, events created on first use
+        DevBuf tiles;
+        cudaEvent_t ev[2]{}; float ms = 0;
+    } retain;
     struct Bodies {                 // request-body rewrite (rows a1-a4) and the document kernels, which share its input staging
         DevBuf plans, ops, blob; uint32_t n_plans = 0, n_ops = 0;       // the rule tables of lgw_rules_load
         DevBuf in, off, out_off, plan_idx, results, scans;      // per call: the packed bodies and five arrays indexed by body
@@ -731,6 +736,44 @@ extern "C" int lgw_usage_latest(lgw_engine* e, const int64_t* d_ts_us, uint64_t 
 extern "C" int lgw_usage_latest_last_ms(lgw_engine* e, float* ms) {
     if (!e || !ms) return LGW_ERR_ARG;
     *ms = e->listing.ms;
+    return LGW_OK;
+}
+
+// ---- deleting old records (tokens_usage_db.py:164-198) ---------------------------------------------------------------------------
+extern "C" int lgw_usage_retain(lgw_engine* e, void* const d_in[8], void* const d_out[8], uint64_t n, int64_t cutoff_us, uint64_t n_keep) {
+    if (!e || n >= (1ull << 32) || n_keep > n) return LGW_ERR_ARG;
+    if (n && (!d_in || !d_out)) return LGW_ERR_ARG;
+    for (int c = 0; n && c < 8; ++c) if (!d_in[c] || (n_keep && !d_out[c])) return LGW_ERR_ARG;
+    if (n && ((uintptr_t)d_in[0] & 15)) return LGW_ERR_ARG;
+    lgw_engine::Retain& rt = e->retain;
+    rt.ms = 0;
+    if (!n) return LGW_OK;
+    CK(e, cudaSetDevice(e->device));
+    const uint32_t N = (uint32_t)n, tiles = (N + LGW_LIST_CTILE - 1) / LGW_LIST_CTILE;
+    CK(e, rt.tiles.reserve(((size_t)tiles + 1) * 4));
+    if (!rt.ev[0]) CK(e, new_events(e, rt.ev, 2));
+    uint32_t* off = rt.tiles.as<uint32_t>();
+    uint32_t* total = off + tiles;
+    RetainCols in{(int64_t*)d_in[0], {}, (double*)d_in[7]}, out{(int64_t*)d_out[0], {}, (double*)d_out[7]};
+    for (int c = 0; c < 6; ++c) { in.i32[c] = (int32_t*)d_in[1 + c]; out.i32[c] = (int32_t*)d_out[1 + c]; }
+    CK(e, cudaEventRecord(rt.ev[0], e->stream));
+    k_retain_count<<<tiles, 1024, 0, e->stream>>>(in.ts, N, cutoff_us, off);
+    k_list_scan<<<1, 1024, 0, e->stream>>>(off, tiles, total);
+    k_retain_write<<<tiles, 1024, 0, e->stream>>>(in, N, cutoff_us, off, (uint32_t)n_keep, out);
+    e->launches += 3;
+    CK(e, cudaEventRecord(rt.ev[1], e->stream));
+    CK(e, cudaGetLastError());
+    uint32_t got = 0;
+    CK(e, cudaMemcpyAsync(&got, total, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    read_ms(rt.ev[0], rt.ev[1], rt.ms);
+    if (got != n_keep) { e->err = "usage retain: " + std::to_string(got) + " records at or after the cutoff, expected " + std::to_string(n_keep); return LGW_ERR_CUDA; }
+    return LGW_OK;
+}
+
+extern "C" int lgw_usage_retain_last_ms(lgw_engine* e, float* ms) {
+    if (!e || !ms) return LGW_ERR_ARG;
+    *ms = e->retain.ms;
     return LGW_OK;
 }
 

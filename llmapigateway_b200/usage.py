@@ -4,6 +4,7 @@ llm_gateway_core/db/tokens_usage_db.py (TokensUsageDB) for rows a10/a11 of SURVE
   UsageTable.insert_usage(d)         <- TokensUsageDB.insert_usage          (:119-162)
   UsageTable.get_aggregated_usage()  <- TokensUsageDB.get_aggregated_usage  (:222-304)  [GPU kernel]
   UsageTable.get_latest_usage_records() <- TokensUsageDB.get_latest_usage_records (:69-117) [GPU kernel: page selection]
+  UsageTable.cleanup_old_records()   <- TokensUsageDB.cleanup_old_records   (:164-198)  [GPU kernel: stable compaction]
   stats_window(period, now)          <- llm_gateway_core/api/v1/stats.py:46-55
 
 Records live as SoA columns (40 B/record) in HBM; `model` is dictionary-encoded at ingest and
@@ -13,9 +14,11 @@ rollup is an integer (see csrc/rollup.cuh), so per-GPU partial tables merge with
 from __future__ import annotations
 
 import ctypes as C
+import logging
 import math
 from datetime import datetime, timedelta
 from fractions import Fraction
+from itertools import compress
 
 import numpy as np
 
@@ -85,6 +88,10 @@ class UsageTable:
 
     COLS = ("ts_us", "model_rank", "prompt_tokens", "completion_tokens", "total_tokens", "reasoning_tokens", "cached_tokens", "cost")
     DTYPES = (np.int64, np.int32, np.int32, np.int32, np.int32, np.int32, np.int32, np.float64)
+    # Record ids, as SQLite's AUTOINCREMENT gives them: _ids holds the id of each host record, a pending row carries its own,
+    # and _seq is the largest id ever given out (sqlite_sequence) -- a deleted id is never given out again.
+    _ids = np.zeros(0, np.int64)
+    _seq = 0
 
     def __init__(self, engine):
         self.eng = engine
@@ -127,7 +134,8 @@ class UsageTable:
         except Exception:
             self.rejected += 1
             return False
-        self._pending_rows.append((ts, model, *counts, cost, provider))
+        self._seq += 1
+        self._pending_rows.append((ts, model, *counts, cost, provider, self._seq))
         self._dev = None
         return True
 
@@ -141,6 +149,8 @@ class UsageTable:
                       "cached_tokens": np.ascontiguousarray(cached, np.int32), "cost": np.ascontiguousarray(cost, np.float64)}
         self._models = list(models)
         self._providers = [None] * len(self._models)
+        self._ids = np.arange(1, len(self._models) + 1, dtype=np.int64)
+        self._seq = len(self._models)
         self._pending_rows = []
         self._dev = None
         self._dev_n = None
@@ -156,6 +166,7 @@ class UsageTable:
             self._host = fresh
             self._models = list(self._models) + list(cols[1])
             self._providers = list(self._providers) + list(cols[8])
+            self._ids = np.concatenate([self._ids, np.array(cols[9], np.int64)])
             self._pending_rows = []
         names = getattr(self, "_fixed_names", None) or sorted({m for m in self._models if m is not None}, key=lambda s: s.encode("utf-8"))
         rank = {m: i + 1 for i, m in enumerate(names)}
@@ -169,8 +180,11 @@ class UsageTable:
         self._dev = None
         self._dev_n = None
         if ptrs and getattr(self.eng, "_h", None):
-            for p in ptrs.values():
-                self._lib.lgw_device_free(self.eng._h, p)
+            self._free_ptrs(ptrs)
+
+    def _free_ptrs(self, ptrs: dict):
+        for p in ptrs.values():
+            self._lib.lgw_device_free(self.eng._h, p)
 
     def close(self):
         self._free_device()
@@ -344,12 +358,12 @@ class UsageTable:
         h = self._host
         n_host = int(h["ts_us"].size)
         if i < n_host:
-            ts, model, provider = int(h["ts_us"][i]), self._models[i], self._providers[i]
+            ts, model, provider, rid = int(h["ts_us"][i]), self._models[i], self._providers[i], int(self._ids[i])
             tok = [int(h[c][i]) for c in self.COLS[2:7]]
             cost = float(h["cost"][i])
         else:
-            ts, model, *tok, cost, provider = self._pending_rows[i - n_host]
-        return {"id": i + 1, "timestamp": (_EPOCH + timedelta(microseconds=int(ts))).isoformat(),
+            ts, model, *tok, cost, provider, rid = self._pending_rows[i - n_host]
+        return {"id": rid, "timestamp": (_EPOCH + timedelta(microseconds=int(ts))).isoformat(),
                 "prompt_tokens": int(tok[0]), "completion_tokens": int(tok[1]), "total_tokens": int(tok[2]),
                 "reasoning_tokens": int(tok[3]), "cached_tokens": int(tok[4]), "cost": _sql_value(float(cost)),
                 "model": model, "provider": provider}
@@ -388,6 +402,81 @@ class UsageTable:
         # every position holds global rank j when lo == 0
         start = offset - lo
         return [self._record(int(i)) for i in merged[start:start + limit]]
+
+    # -- deleting old records (tokens_usage_db.py:164-198) ---------------------------------------------------------------
+    def cleanup_old_records(self, retention_days: int = 180, now: datetime | None = None) -> None:
+        """tokens_usage_db.py:164-198: delete the records older than `now - retention_days` (`now` defaults to
+        datetime.now()).  A record goes exactly when ts_us < to_us(cutoff); one at the cutoff stays.  For every timestamp a
+        datetime can express this is SQLite's `timestamp < cutoff.isoformat()` on the text (isoformat drops a zero microsecond
+        part, which sorts the same); timestamps with no text form (only load_columns can give them, e.g. INT64_MIN) compare as
+        the integers they are.  Ids survive, and the next insert gets the largest id ever given out + 1, as AUTOINCREMENT does.
+        Like the reference this never raises and returns None: a bad `retention_days`, a cutoff outside datetime's range or a
+        failed device call is logged and deletes nothing.  Uploaded records are compacted on the device (_retain_on_device);
+        the table stays resident, model names keep their ranks until the next re-rank, and nothing is uploaded again."""
+        try:
+            cutoff = to_us((now if now is not None else datetime.now()) - timedelta(days=retention_days))
+            deleted = self._retain(cutoff)
+        except Exception as e:
+            logging.error(f"Error cleaning up old token usage records: {str(e)}")
+            return None
+        if deleted > 0:
+            logging.info(f"Cleaned up {deleted} old token usage records (older than {retention_days} days)")
+        else:
+            logging.debug("No old token usage records to clean up")
+        return None
+
+    def _retain(self, cutoff: int) -> int:
+        """delete every record with ts_us < cutoff; the number deleted.  The device call comes first: if it fails, host and
+        device are as they were.  Rows not on the device (host rows past _dev_n, pending rows) are deleted on the host only."""
+        h = self._host
+        keep = h["ts_us"] >= cutoff
+        pend_keep = [r[0] >= cutoff for r in self._pending_rows]
+        deleted = int(keep.size - np.count_nonzero(keep)) + pend_keep.count(False)
+        if deleted == 0:
+            return 0
+        n_dev = self._dev_n
+        if n_dev is not None:
+            n_keep = int(np.count_nonzero(keep[:n_dev]))
+            if n_keep < n_dev:
+                fresh = self._retain_on_device(n_dev, cutoff, n_keep)
+                old, self._dev_ptrs = self._dev_ptrs, fresh
+                self._free_ptrs(old)
+                if self._dev is not None:
+                    self._dev = (n_keep, fresh)
+                self._dev_n = n_keep
+        idx = np.flatnonzero(keep)                # (take() with indices is several times faster than a boolean mask here)
+        self._host = {c: (a.take(idx) if a is not None else None) for c, a in h.items()}
+        self._ids = self._ids.take(idx)
+        mask = keep.tolist()                      # (compress() over a list of bools, not over numpy bools: far faster)
+        self._models = list(compress(self._models, mask))
+        self._providers = list(compress(self._providers, mask))
+        self._pending_rows = list(compress(self._pending_rows, pend_keep))
+        return deleted
+
+    def _retain_on_device(self, n: int, cutoff: int, n_keep: int) -> dict:
+        """the n uploaded records with ts_us >= cutoff, compacted into fresh device columns (lgw_usage_retain); the old
+        columns stay as they were, and on a failure the fresh ones are freed"""
+        lib, h = self._lib, self.eng._h
+        fresh = {}
+        try:
+            for c, d in zip(self.COLS, self.DTYPES):
+                p = C.c_void_p()
+                self.eng._ck(lib.lgw_device_alloc(h, max(n_keep * np.dtype(d).itemsize, 8), C.byref(p)), "device_alloc")
+                fresh[c] = p
+            src = (C.c_void_p * 8)(*[self._dev_ptrs[c].value for c in self.COLS])
+            dst = (C.c_void_p * 8)(*[fresh[c].value for c in self.COLS])
+            self.eng._ck(lib.lgw_usage_retain(h, src, dst, n, cutoff, n_keep), "usage_retain")
+        except BaseException:
+            self._free_ptrs(fresh)
+            raise
+        return fresh
+
+    def retain_last_ms(self) -> float:
+        """device time of the last lgw_usage_retain, milliseconds (a cleanup that deletes no uploaded record makes no device
+        call and leaves it as it was)"""
+        ms = C.c_float()
+        self.eng._ck(self._lib.lgw_usage_retain_last_ms(self.eng._h, C.byref(ms)), "usage_retain_last_ms")
+        return ms.value
 
     def last_ms(self):
         ms = (C.c_float * 2)()
