@@ -13,6 +13,7 @@
 #include <cuda_runtime.h>
 #include "body_machine.cuh"
 #include "body_fast.cuh"
+#include "scan.cuh"
 
 namespace lgw {
 
@@ -84,32 +85,11 @@ k_body_rewrite(const uint8_t* __restrict__ bodies, const uint64_t* __restrict__ 
 // exclusive scan over the OK lengths; one block, n is small (thousands) compared with the bodies
 __global__ void __launch_bounds__(1024)
 k_body_offsets(const BodyResult* __restrict__ results, uint32_t n, uint64_t out_cap, uint64_t* __restrict__ out_off) {
-    __shared__ uint64_t warp_sum[32];
-    __shared__ uint64_t base;
-    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
-    if (threadIdx.x == 0) base = 0;
-    __syncthreads();
-    for (uint32_t start = 0; start < n; start += 1024) {
-        const uint32_t i = start + threadIdx.x;
-        uint64_t v = 0;
-        if (i < n) { const BodyResult r = results[i]; v = r.status == BS_OK ? r.out_len : 0; }
-        uint64_t s = v;
-        for (int d = 1; d < 32; d <<= 1) { const uint64_t t = __shfl_up_sync(0xffffffffu, s, d); if (lane >= (uint32_t)d) s += t; }
-        if (lane == 31) warp_sum[w] = s;
-        __syncthreads();
-        if (w == 0) {
-            uint64_t ws = warp_sum[lane], t2 = ws;
-            for (int d = 1; d < 32; d <<= 1) { const uint64_t t = __shfl_up_sync(0xffffffffu, t2, d); if (lane >= (uint32_t)d) t2 += t; }
-            warp_sum[lane] = t2 - ws;
-        }
-        __syncthreads();
-        const uint64_t excl = base + warp_sum[w] + s - v;
-        if (i < n) out_off[i] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023 || i == n - 1) { base = excl + v; }
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) out_off[n] = base;
+    __shared__ WarpSums<uint64_t> warp_sums;
+    const uint64_t total = block_scan(n, threadIdx.x, blockDim.x, warp_sums,
+                                      [&](uint32_t i) { const BodyResult r = results[i]; return r.status == BS_OK ? r.out_len : 0u; },
+                                      [&](uint32_t i, uint64_t off) { out_off[i] = off; });
+    if (threadIdx.x == 0) out_off[n] = total;
 }
 
 __global__ void __launch_bounds__(256)

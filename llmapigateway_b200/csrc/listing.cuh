@@ -17,6 +17,8 @@
 #pragma once
 #include <stdint.h>
 
+#include "scan.cuh"
+
 namespace lgw {
 
 #define LGW_LIST_CAND_DIV 16u        /* compact the candidates once they are at most n / 16 */
@@ -166,69 +168,55 @@ __device__ __forceinline__ void list_load_pair(const int64_t* __restrict__ ts, u
     else if (2 * j < n) a = __ldg(ts + 2 * j);
 }
 
-// records of each compaction tile between the two boundaries
-__global__ void __launch_bounds__(1024) k_list_tile_count(const int64_t* __restrict__ ts, uint32_t n, const ListSel* __restrict__ sp, uint32_t* __restrict__ tile_count) {
-    __shared__ uint32_t warp_sums[32];
-    const ListSel s = *sp;
+// Ordered compaction of a timestamp column in tiles of LGW_LIST_CTILE records (1024 threads, one 16-byte load each), shared by
+// the listing and retain.cuh: keep(ts, index) picks the records.  ctile_count writes the number of kept records of each tile;
+// after an exclusive scan of the counts (k_list_scan), ctile_write hands each kept record to store(index, ts, place) in index
+// order.  Places at or past cap are not stored: a count that differs from the caller's is caught by the host's check of the
+// scan's total, never by writing past the output.
+template <class Keep>
+__device__ __forceinline__ void ctile_count(const int64_t* __restrict__ ts, uint32_t n, Keep keep, uint32_t* __restrict__ tile_count) {
+    __shared__ WarpSums<uint32_t> warp_sums;
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     int64_t a, b;
     list_load_pair(ts, n, j, a, b);
-    const uint32_t c = (2 * j < n && list_between(list_key(a), 2 * j, s)) + (2 * j + 1 < n && list_between(list_key(b), 2 * j + 1, s));
-    const uint32_t w = __reduce_add_sync(0xFFFFFFFFu, c);
-    if ((threadIdx.x & 31u) == 0) warp_sums[threadIdx.x >> 5] = w;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        const uint32_t t = __reduce_add_sync(0xFFFFFFFFu, threadIdx.x < (blockDim.x >> 5) ? warp_sums[threadIdx.x] : 0u);
-        if (threadIdx.x == 0) tile_count[blockIdx.x] = t;
-    }
+    const uint32_t c = block_sum((2 * j < n && keep(a, 2 * j)) + (2 * j + 1 < n && keep(b, 2 * j + 1)), threadIdx.x, blockDim.x, warp_sums);
+    if (threadIdx.x == 0) tile_count[blockIdx.x] = c;
+}
+
+template <class Keep, class Store>
+__device__ __forceinline__ void ctile_write(const int64_t* __restrict__ ts, uint32_t n, Keep keep, const uint32_t* __restrict__ tile_off, uint32_t cap, Store store) {
+    __shared__ WarpSums<uint32_t> warp_sums;
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t a, b;
+    list_load_pair(ts, n, j, a, b);
+    const bool ka = 2 * j < n && keep(a, 2 * j), kb = 2 * j + 1 < n && keep(b, 2 * j + 1);
+    uint32_t pos = tile_off[blockIdx.x] + warp_place(ka, kb, threadIdx.x, warp_sums);
+    if (ka) { if (pos < cap) store(2 * j, a, pos); ++pos; }
+    if (kb && pos < cap) store(2 * j + 1, b, pos);
+}
+
+// records of each compaction tile between the two boundaries
+__global__ void __launch_bounds__(1024) k_list_tile_count(const int64_t* __restrict__ ts, uint32_t n, const ListSel* __restrict__ sp, uint32_t* __restrict__ tile_count) {
+    const ListSel s = *sp;
+    ctile_count(ts, n, [&](int64_t t, uint32_t i) { return list_between(list_key(t), i, s); }, tile_count);
 }
 
 // exclusive scan in place of column blockIdx.x (len entries at v + blockIdx.x * len); the column's total to totals[blockIdx.x]
 __global__ void __launch_bounds__(1024) k_list_scan(uint32_t* v, uint32_t len, uint32_t* totals) {
-    __shared__ uint32_t warp_sums[32];
-    __shared__ uint32_t base;
+    __shared__ WarpSums<uint32_t> warp_sums;
     uint32_t* col = v + (size_t)blockIdx.x * len;
-    if (threadIdx.x == 0) base = 0;
-    __syncthreads();
-    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    for (uint32_t start = 0; start < len; start += blockDim.x) {
-        const uint32_t k = start + threadIdx.x;
-        const uint32_t x0 = k < len ? col[k] : 0u;
-        uint32_t x = x0;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= (uint32_t)d) x += y; }
-        if (lane == 31) warp_sums[warp] = x;
-        __syncthreads();
-        uint32_t before = 0, all = 0;
-        for (uint32_t w = 0; w < (blockDim.x >> 5); ++w) { const uint32_t t = warp_sums[w]; if (w < warp) before += t; all += t; }
-        if (k < len) col[k] = base + before + x - x0;
-        __syncthreads();
-        if (threadIdx.x == 0) base += all;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) totals[blockIdx.x] = base;
+    const uint32_t total = block_scan(len, threadIdx.x, blockDim.x, warp_sums, [&](uint32_t k) { return col[k]; },
+                                      [&](uint32_t k, uint32_t off) { col[k] = off; });
+    if (threadIdx.x == 0) totals[blockIdx.x] = total;
 }
 
 // the keys between the two boundaries, in index order, at the tile offsets k_list_scan made.  Only the first `count` are stored:
-// keys / idx hold `count` entries, and a selection that put more records between the boundaries is caught by the host's check
-// of the total (k_list_scan's), not by writing past them into the rest of the scratch.
+// keys / idx hold `count` entries.
 __global__ void __launch_bounds__(1024) k_list_tile_write(const int64_t* __restrict__ ts, uint32_t n, const ListSel* __restrict__ sp, const uint32_t* __restrict__ tile_off,
                                                           uint32_t count, uint64_t* __restrict__ keys, uint32_t* __restrict__ idx) {
-    __shared__ uint32_t warp_sums[32];
     const ListSel s = *sp;
-    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, lt = (1u << lane) - 1u;
-    int64_t a, b;
-    list_load_pair(ts, n, j, a, b);
-    const uint64_t ka = list_key(a), kb = list_key(b);
-    const bool ia = 2 * j < n && list_between(ka, 2 * j, s), ib = 2 * j + 1 < n && list_between(kb, 2 * j + 1, s);
-    const uint32_t ma = __ballot_sync(0xFFFFFFFFu, ia), mb = __ballot_sync(0xFFFFFFFFu, ib);
-    if (lane == 0) warp_sums[warp] = __popc(ma) + __popc(mb);
-    __syncthreads();
-    uint32_t pos = tile_off[blockIdx.x] + __popc(ma & lt) + __popc(mb & lt);
-    for (uint32_t w = 0; w < warp; ++w) pos += warp_sums[w];
-    if (ia) { if (pos < count) { keys[pos] = ka; idx[pos] = 2 * j; } ++pos; }
-    if (ib && pos < count) { keys[pos] = kb; idx[pos] = 2 * j + 1; }
+    ctile_write(ts, n, [&](int64_t t, uint32_t i) { return list_between(list_key(t), i, s); }, tile_off, count,
+               [&](uint32_t i, int64_t t, uint32_t pos) { keys[pos] = list_key(t); idx[pos] = i; });
 }
 
 // pages up to LGW_LIST_SMEM_SORT: bitonic sort of (kd, index) in shared memory by one block; indices out as uint64
@@ -281,20 +269,11 @@ __global__ void __launch_bounds__(256) k_lsd_scatter(const uint64_t* __restrict_
     __shared__ uint32_t run[256];
     __shared__ uint32_t wcnt[8][256];                 // (round + 1) << 8 | lanes of warp w with the digit, this round
     __shared__ uint32_t wpre[8][256];
-    __shared__ uint32_t wsum[8];
+    __shared__ WarpSums<uint32_t> warp_sums;
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, lt = (1u << lane) - 1u;
     for (uint32_t w = 0; w < 8; ++w) wcnt[w][threadIdx.x] = 0;
-    {   // run[d] = keys of digits below d (exclusive scan of the totals) + this tile's offset within digit d
-        const uint32_t t = totals[threadIdx.x];
-        uint32_t x = t;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= (uint32_t)d) x += y; }
-        if (lane == 31) wsum[warp] = x;
-        __syncthreads();
-        uint32_t before = 0;
-        for (uint32_t w = 0; w < warp; ++w) before += wsum[w];
-        run[threadIdx.x] = before + x - t + tile_off[(size_t)threadIdx.x * n_tiles + blockIdx.x];
-    }
+    uint32_t all;                                      // run[d] = keys of digits below d + this tile's offset within digit d
+    run[threadIdx.x] = block_exclusive_scan(totals[threadIdx.x], threadIdx.x, 256, warp_sums, all) + tile_off[(size_t)threadIdx.x * n_tiles + blockIdx.x];
     __syncthreads();
     for (uint32_t r = 0; r < LGW_LIST_STILE / 256; ++r) {
         const uint32_t i = blockIdx.x * LGW_LIST_STILE + r * 256 + threadIdx.x;

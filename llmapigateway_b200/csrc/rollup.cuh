@@ -21,6 +21,7 @@
 
 #if defined(__CUDACC__)
 #define LGW_RHD __host__ __device__ __forceinline__
+#include "scan.cuh"                  // for the kernels, which only the CUDA build has
 #else
 #define LGW_RHD inline
 #endif
@@ -314,43 +315,20 @@ __global__ void __launch_bounds__(1024) k_rollup_count(const unsigned long long*
 }
 
 __global__ void __launch_bounds__(1024) k_rollup_scan(uint32_t* tile_count, uint32_t n_tiles, unsigned long long* n_rows) {
-    __shared__ uint32_t warp_sums[32];
-    __shared__ uint32_t base;
-    if (threadIdx.x == 0) base = 0;
-    __syncthreads();
-    for (uint32_t start = 0; start < n_tiles; start += blockDim.x) {
-        const uint32_t k = start + threadIdx.x;
-        const uint32_t v = k < n_tiles ? tile_count[k] : 0;
-        uint32_t x = v;                                               // inclusive warp scan
-        const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= (uint32_t)d) x += y; }
-        if (lane == 31) warp_sums[warp] = x;
-        __syncthreads();
-        uint32_t before = 0, all = 0;
-        for (uint32_t w = 0; w < 32; ++w) { const uint32_t s = warp_sums[w]; if (w < warp) before += s; all += s; }
-        if (k < n_tiles) tile_count[k] = base + before + x - v;       // exclusive offset of the tile
-        __syncthreads();
-        if (threadIdx.x == 0) base += all;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *n_rows = base;
+    __shared__ WarpSums<uint32_t> warp_sums;
+    const uint32_t total = block_scan(n_tiles, threadIdx.x, blockDim.x, warp_sums, [&](uint32_t k) { return tile_count[k]; },
+                                      [&](uint32_t k, uint32_t off) { tile_count[k] = off; });
+    if (threadIdx.x == 0) *n_rows = total;
 }
 
 __global__ void __launch_bounds__(1024) k_rollup_write(const unsigned long long* __restrict__ table, const uint32_t* __restrict__ inexact, uint32_t n_buckets, uint32_t n_models,
                                                        int64_t bucket0, const uint32_t* __restrict__ tile_off, RollupRow* rows, unsigned long long rows_cap) {
-    __shared__ uint32_t warp_sums[32];
+    __shared__ WarpSums<uint32_t> warp_sums;
     const uint64_t total = (uint64_t)n_buckets * n_models;
     const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     uint64_t g = 0; uint32_t has = 0;
     if (j < total) { g = rollup_group_at(j, n_buckets, n_models); has = table[g * LGW_ROLLUP_CELLS + 5] != 0; }
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t ballot = __ballot_sync(0xFFFFFFFFu, has);
-    if (lane == 0) warp_sums[warp] = __popc(ballot);
-    __syncthreads();
-    uint32_t before = 0;
-    for (uint32_t w = 0; w < warp; ++w) before += warp_sums[w];
-    const unsigned long long pos = (unsigned long long)tile_off[blockIdx.x] + before + __popc(ballot & ((1u << lane) - 1));
+    const unsigned long long pos = (unsigned long long)tile_off[blockIdx.x] + warp_place(has, false, threadIdx.x, warp_sums);
     if (has && pos < rows_cap) {
         const unsigned long long* c = table + g * LGW_ROLLUP_CELLS;
         RollupRow r;

@@ -23,6 +23,7 @@
 // Host/device portable like stream_machine.cuh (tests compile it with g++ over the SIMT emulator; the product has no CPU path).
 #pragma once
 #include "stream_machine.cuh"
+#include "scan.cuh"
 
 namespace lgw {
 
@@ -289,31 +290,10 @@ k_text_extract(TextArgs a) {
 
 // exclusive scan of seg_len -> seg_off[0 .. n_segs] (one block of 1024 threads)
 TX_GLOBAL void k_text_scan(const uint32_t* seg_len, uint32_t n_segs, unsigned long long* seg_off) {
-    TX_SHARED unsigned long long warp_sum[32];
-    TX_SHARED unsigned long long carry_s;
-    const uint32_t tid = TX_TID, lane = tid & 31u, w = tid >> 5;
-    if (tid == 0) carry_s = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < n_segs; base += TX_NTHR) {
-        const uint32_t i = base + tid;
-        const unsigned long long v = i < n_segs ? seg_len[i] : 0;
-        unsigned long long x = v;
-        for (uint32_t d = 1; d < 32; d <<= 1) { const unsigned long long y = __shfl_up_sync(TX_FULL, x, d); if (lane >= d) x += y; }
-        if (lane == 31) warp_sum[w] = x;
-        __syncthreads();
-        if (w == 0) {
-            unsigned long long s = lane < (TX_NTHR >> 5) ? warp_sum[lane] : 0;
-            for (uint32_t d = 1; d < 32; d <<= 1) { const unsigned long long y = __shfl_up_sync(TX_FULL, s, d); if (lane >= d) s += y; }
-            warp_sum[lane] = s;
-        }
-        __syncthreads();
-        const unsigned long long before = carry_s + (w ? warp_sum[w - 1] : 0) + (x - v);
-        if (i < n_segs) seg_off[i] = before;
-        __syncthreads();
-        if (tid == TX_NTHR - 1) carry_s = before + v;
-        __syncthreads();
-    }
-    if (tid == 0) seg_off[n_segs] = carry_s;
+    TX_SHARED WarpSums<unsigned long long> warp_sums;
+    const unsigned long long total = block_scan(n_segs, TX_TID, TX_NTHR, warp_sums, [&](uint32_t i) { return seg_len[i]; },
+                                                [&](uint32_t i, unsigned long long off) { seg_off[i] = off; });
+    if (TX_TID == 0) seg_off[n_segs] = total;
 }
 
 // compaction: the pieces of segment s, in chunk order, to text[seg_off[s] ..)
