@@ -263,6 +263,22 @@ int lgw_usage_retain(lgw_engine* e, void* const d_in[8], void* const d_out[8], u
 /* device time of the last lgw_usage_retain, milliseconds (0 after a call with n == 0) */
 int lgw_usage_retain_last_ms(lgw_engine* e, float* ms);
 
+/* insert_usage (tokens_usage_db.py:119-162) on the device copy: m new records appended after the n resident ones.  Columns in
+ * UsageTable.COLS order, typed as lgw_usage_retain's.  d_cols holds the n resident records; h_new the m new ones in host
+ * memory, their model_rank final.  d_grow == NULL: the new rows go to d_cols[c] + n (the caller guarantees room for n + m);
+ * else d_grow are fresh columns with room for n + m, not overlapping d_cols, and records [0, n) are copied into them first.
+ * rank_map (host, n_map entries, or NULL): a resident record's model_rank r becomes rank_map[r], in place or while it is
+ * copied.  A resident rank >= n_map (or negative) is counted on the device and fails the call (LGW_ERR_CUDA, message in
+ * lgw_last_error); that record keeps its rank.  Nothing is written outside [0, n + m) of the target columns.  n + m >= 2^32,
+ * a null pointer that the call needs, a ts_us column (d_cols or d_grow) that is not 16-byte aligned, or rank_map with
+ * n_map == 0: LGW_ERR_ARG.  m == 0 with neither a map nor d_grow launches nothing.
+ * Device work: one host-to-device copy of the new rows and the map through engine-owned page-locked staging, and one launch of
+ * k_usage_append (csrc/append.cuh).  The call returns when the columns are written. */
+int lgw_usage_append(lgw_engine* e, void* const d_cols[8], void* const d_grow[8], uint64_t n,
+                     const void* const h_new[8], uint64_t m, const int32_t* rank_map, uint32_t n_map);
+/* device time of the last lgw_usage_append (its copy and kernel), milliseconds (0 after a call that launched nothing) */
+int lgw_usage_append_last_ms(lgw_engine* e, float* ms);
+
 /* ---- request-body rewrite: SURVEY 8 rows a1, a3, a4 --------------------------------------------------
  * Replaces, for a batch of client requests, chat.py:31-45 (parse: lgw_bodies_scan) and, per upstream
  * attempt, chat.py:112-119,:135-139,:150,:164-168 (deepcopy + key assignments) followed by the encoder

@@ -12,6 +12,7 @@
 #include "rollup.cuh"
 #include "listing.cuh"
 #include "retain.cuh"
+#include "append.cuh"
 #include "body_kernels.cuh"
 #include "doc_kernels.cuh"
 #include "transcript.cuh"
@@ -43,6 +44,24 @@ struct DevBuf {
         if (p) cudaFree(p);
         p = nullptr; cap = 0;
         const cudaError_t r = cudaMalloc(&p, need + slack);
+        if (r == cudaSuccess) cap = need + slack;
+        return r;
+    }
+    template <class T> T* as() const { return static_cast<T*>(p); }
+};
+
+// The same for page-locked host staging (cudaHostAlloc).
+struct HostBuf {
+    void* p = nullptr; size_t cap = 0;
+    HostBuf() = default;
+    HostBuf(const HostBuf&) = delete;
+    HostBuf& operator=(const HostBuf&) = delete;
+    ~HostBuf() { if (p) cudaFreeHost(p); }
+    cudaError_t reserve(size_t need, size_t slack = 0) {
+        if (need <= cap) return cudaSuccess;
+        if (p) cudaFreeHost(p);
+        p = nullptr; cap = 0;
+        const cudaError_t r = cudaHostAlloc(&p, need + slack, cudaHostAllocDefault);
         if (r == cudaSuccess) cap = need + slack;
         return r;
     }
@@ -107,6 +126,10 @@ struct lgw_engine {
         DevBuf tiles;
         cudaEvent_t ev[2]{}; float ms = 0;
     } retain;
+    struct Append {                 // inserted records (append.cuh): the new rows and the rank map, staged page-locked, then on the device
+        HostBuf host; DevBuf dev;
+        cudaEvent_t ev[2]{}; float ms = 0;
+    } append;
     struct Bodies {                 // request-body rewrite (rows a1-a4) and the document kernels, which share its input staging
         DevBuf plans, ops, blob; uint32_t n_plans = 0, n_ops = 0;       // the rule tables of lgw_rules_load
         DevBuf in, off, out_off, plan_idx, results, scans;      // per call: the packed bodies and five arrays indexed by body
@@ -774,6 +797,75 @@ extern "C" int lgw_usage_retain(lgw_engine* e, void* const d_in[8], void* const 
 extern "C" int lgw_usage_retain_last_ms(lgw_engine* e, float* ms) {
     if (!e || !ms) return LGW_ERR_ARG;
     *ms = e->retain.ms;
+    return LGW_OK;
+}
+
+// ---- inserted records (tokens_usage_db.py:119-162) -------------------------------------------------------------------------------
+extern "C" int lgw_usage_append(lgw_engine* e, void* const d_cols[8], void* const d_grow[8], uint64_t n,
+                                const void* const h_new[8], uint64_t m, const int32_t* rank_map, uint32_t n_map) {
+    if (!e || n >= (1ull << 32) || m >= (1ull << 32) || n + m >= (1ull << 32) || (rank_map && n_map == 0)) return LGW_ERR_ARG;
+    const bool grow = d_grow != nullptr, remap = rank_map != nullptr;
+    const uint64_t old = (grow || remap) ? n : 0;
+    const bool need_cols = old > 0 || (!grow && m > 0);            // d_cols is read, or written in place
+    if (need_cols) {
+        if (!d_cols) return LGW_ERR_ARG;
+        for (int c = 0; c < 8; ++c) if (!d_cols[c]) return LGW_ERR_ARG;
+        if ((uintptr_t)d_cols[0] & 15) return LGW_ERR_ARG;
+    }
+    if (grow && old + m > 0) {
+        for (int c = 0; c < 8; ++c) if (!d_grow[c]) return LGW_ERR_ARG;
+        if ((uintptr_t)d_grow[0] & 15) return LGW_ERR_ARG;
+    }
+    if (m && !h_new) return LGW_ERR_ARG;
+    for (int c = 0; m && c < 8; ++c) if (!h_new[c]) return LGW_ERR_ARG;
+    lgw_engine::Append& ap = e->append;
+    ap.ms = 0;
+    if (old + m == 0) return LGW_OK;
+    CK(e, cudaSetDevice(e->device));
+    // staging: m timestamps, m costs, the six int32 columns, the map, the bad-rank counter (zero, copied up with the rest)
+    const size_t o_cost = 8 * m, o_i32 = 16 * m, o_map = 40 * m, o_bad = o_map + (remap ? 4ull * n_map : 0), bytes = o_bad + 4;
+    CK(e, ap.host.reserve(bytes, bytes / 4 + 4096));
+    CK(e, ap.dev.reserve(bytes, bytes / 4 + 4096));
+    if (!ap.ev[0]) CK(e, new_events(e, ap.ev, 2));
+    uint8_t* st = ap.host.as<uint8_t>();
+    if (m) {
+        memcpy(st, h_new[0], 8 * m);
+        memcpy(st + o_cost, h_new[7], 8 * m);
+        for (int c = 0; c < 6; ++c) memcpy(st + o_i32 + 4 * m * c, h_new[1 + c], 4 * m);
+    }
+    if (remap) memcpy(st + o_map, rank_map, 4ull * n_map);
+    memset(st + o_bad, 0, 4);
+    uint8_t* dv = ap.dev.as<uint8_t>();
+    void* const* dst = grow ? d_grow : d_cols;
+    AppendArgs a{};
+    if (need_cols) {
+        a.src.ts = (int64_t*)d_cols[0]; a.src.cost = (double*)d_cols[7];
+        for (int c = 0; c < 6; ++c) a.src.i32[c] = (int32_t*)d_cols[1 + c];
+    }
+    a.dst.ts = (int64_t*)dst[0]; a.dst.cost = (double*)dst[7];
+    for (int c = 0; c < 6; ++c) a.dst.i32[c] = (int32_t*)dst[1 + c];
+    if (!grow) a.src = a.dst;
+    a.new_ts = (const int64_t*)dv; a.new_cost = (const double*)(dv + o_cost); a.new_i32 = (const int32_t*)(dv + o_i32);
+    a.map = remap ? (const int32_t*)(dv + o_map) : nullptr;
+    a.n_map = remap ? n_map : 0; a.n = (uint32_t)n; a.m = (uint32_t)m; a.old = (uint32_t)old;
+    a.bad = (uint32_t*)(dv + o_bad);
+    CK(e, cudaEventRecord(ap.ev[0], e->stream));
+    CK(e, cudaMemcpyAsync(dv, st, bytes, cudaMemcpyHostToDevice, e->stream));
+    k_usage_append<<<grid_for(e, old + m, 256, 8), 256, 0, e->stream>>>(a);
+    ++e->launches;
+    CK(e, cudaEventRecord(ap.ev[1], e->stream));
+    CK(e, cudaGetLastError());
+    uint32_t bad = 0;
+    CK(e, cudaMemcpyAsync(&bad, a.bad, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    read_ms(ap.ev[0], ap.ev[1], ap.ms);
+    if (bad) { e->err = "usage append: " + std::to_string(bad) + " resident model ranks at or past the map's " + std::to_string(n_map) + " entries"; return LGW_ERR_CUDA; }
+    return LGW_OK;
+}
+
+extern "C" int lgw_usage_append_last_ms(lgw_engine* e, float* ms) {
+    if (!e || !ms) return LGW_ERR_ARG;
+    *ms = e->append.ms;
     return LGW_OK;
 }
 

@@ -1,7 +1,7 @@
 """Usage records on the device and their rollup -- the host-side mirror of
 llm_gateway_core/db/tokens_usage_db.py (TokensUsageDB) for rows a10/a11 of SURVEY.md section 8:
 
-  UsageTable.insert_usage(d)         <- TokensUsageDB.insert_usage          (:119-162)
+  UsageTable.insert_usage(d)         <- TokensUsageDB.insert_usage          (:119-162)  [GPU kernel: append at query time]
   UsageTable.get_aggregated_usage()  <- TokensUsageDB.get_aggregated_usage  (:222-304)  [GPU kernel]
   UsageTable.get_latest_usage_records() <- TokensUsageDB.get_latest_usage_records (:69-117) [GPU kernel: page selection]
   UsageTable.cleanup_old_records()   <- TokensUsageDB.cleanup_old_records   (:164-198)  [GPU kernel: stable compaction]
@@ -29,6 +29,7 @@ _EPOCH = datetime(1970, 1, 1)
 ROLLUP_CELLS = 10
 # the record listing merges up to this many rows inserted since the last upload on the host; more, and it uploads the table again
 LISTING_PENDING_MAX = 65536
+APPEND_MAX = (1 << 32) - 1      # records a device table can hold (lgw_usage_append: n + m < 2^32)
 
 ROW_DTYPE = np.dtype([("bucket", "<i8"), ("model_rank", "<i4"), ("inexact", "<u4"), ("prompt_tokens", "<i8"),
                       ("completion_tokens", "<i8"), ("total_tokens", "<i8"), ("reasoning_tokens", "<i8"),
@@ -92,6 +93,18 @@ class UsageTable:
     # and _seq is the largest id ever given out (sqlite_sequence) -- a deleted id is never given out again.
     _ids = np.zeros(0, np.int64)
     _seq = 0
+    # Inserts append: _rank (model name -> rank, None: rank every record at the next _materialise) persists between
+    # materialisations; _hbuf holds the buffers the host columns and ids are exact-length views of, with room to grow;
+    # _dev_rank_map maps the ranks of the resident device records to the current ones when a new name shifted them (None: no
+    # shift since the device was last brought up to date); _dev_cap is the capacity of the device columns, in records;
+    # _ts_range is (the ts_us array it describes, min, max), kept across inserts so that a rollup needs no pass over the column.
+    _rank = None
+    _fixed_names = None
+    _hbuf = None
+    _dev_n = None
+    _dev_rank_map = None
+    _dev_cap = 0
+    _ts_range = None
 
     def __init__(self, engine):
         self.eng = engine
@@ -154,31 +167,87 @@ class UsageTable:
         self._pending_rows = []
         self._dev = None
         self._dev_n = None
+        self._rank = None
+        self._dev_rank_map = None
+        self._ts_range = None
+
+    def _grow(self, key: str, a: np.ndarray, new: np.ndarray) -> np.ndarray:
+        """a followed by new, as an exact-length view of a buffer of this table with room to grow (doubling): when a is the
+        view of that buffer and it has room, the values already there are not touched"""
+        if self._hbuf is None:
+            self._hbuf = {}
+        n, m = a.size, new.size
+        buf = self._hbuf.get(key)
+        if buf is None or a.base is not buf or n + m > buf.size:
+            buf = self._hbuf[key] = np.empty(max(2 * (n + m), 1024), a.dtype)
+            buf[:n] = a
+        buf[n:n + m] = new
+        return buf[:n + m]
 
     def _materialise(self):
+        """Move the pending rows into the host columns and rank their model names.  Only the new rows are visited, except
+        when a new name shifts the ranks of the old ones (see _rank_new)."""
         if self._pending_rows:
             cols = list(zip(*self._pending_rows))
             h = self._host
-            fresh = {"ts_us": np.concatenate([h["ts_us"], np.array(cols[0], np.int64)]), "model_rank": None}     # built completely
-            for k, name in enumerate(self.COLS[2:7]):                                                           # before anything
-                fresh[name] = np.concatenate([h[name], np.array(cols[2 + k], np.int32)])                        # is replaced
-            fresh["cost"] = np.concatenate([h["cost"], np.array(cols[7], np.float64)])
+            new = {"ts_us": np.array(cols[0], np.int64), "cost": np.array(cols[7], np.float64)}      # built completely
+            for k, name in enumerate(self.COLS[2:7]):                                                  # before anything is
+                new[name] = np.array(cols[2 + k], np.int32)                                            # replaced
+            ids = np.array(cols[9], np.int64)
+            fresh = {c: (self._grow(c, h[c], new[c]) if c in new else h[c]) for c in self.COLS}
+            self._ids = self._grow("ids", self._ids, ids)
             self._host = fresh
-            self._models = list(self._models) + list(cols[1])
-            self._providers = list(self._providers) + list(cols[8])
-            self._ids = np.concatenate([self._ids, np.array(cols[9], np.int64)])
+            rng, t = self._ts_range, new["ts_us"]
+            if h["ts_us"].size == 0:
+                rng = (fresh["ts_us"], int(t.min()), int(t.max()))
+            elif rng is not None and rng[0] is h["ts_us"]:
+                rng = (fresh["ts_us"], min(rng[1], int(t.min())), max(rng[2], int(t.max())))
+            self._ts_range = rng if rng is not None and rng[0] is fresh["ts_us"] else None
+            self._models.extend(cols[1])
+            self._providers.extend(cols[8])
             self._pending_rows = []
-        names = getattr(self, "_fixed_names", None) or sorted({m for m in self._models if m is not None}, key=lambda s: s.encode("utf-8"))
+        mr = self._host["model_rank"]
+        if mr is None or self._rank is None:
+            self._rank_all()
+        elif mr.size < len(self._models):
+            self._rank_new(mr)
+
+    def _rank_all(self):
+        """rank every record's model name (a table loaded with load_columns, or one never ranked)"""
+        names = self._fixed_names or sorted({m for m in self._models if m is not None}, key=lambda s: s.encode("utf-8"))
         rank = {m: i + 1 for i, m in enumerate(names)}
         rank[None] = 0
         self._host["model_rank"] = np.fromiter((rank[m] for m in self._models), dtype=np.int32, count=len(self._models))
         self._names = [None] + names
+        self._rank = rank
+
+    def _rank_new(self, mr: np.ndarray):
+        """rank the records [mr.size, n) whose names have no rank yet.  A name not ranked before is merged into the byte-ordered
+        names; when that moves an old name, the host ranks are rewritten through the old -> new map and the map is kept for the
+        device records (_dev_rank_map).  A table with a fixed dictionary (load_columns(names=...)) never adds a name."""
+        new_models = self._models[mr.size:]
+        rank = self._rank
+        if not self._fixed_names:
+            unranked = {m for m in new_models if m not in rank}
+            if unranked:
+                old_names = self._names
+                self._names = [None] + sorted(old_names[1:] + list(unranked), key=lambda s: s.encode("utf-8"))
+                rank = self._rank = {m: i for i, m in enumerate(self._names)}
+                step = np.fromiter((rank[m] for m in old_names), dtype=np.int32, count=len(old_names))
+                if np.any(step != np.arange(len(old_names), dtype=np.int32)):
+                    mr[...] = step[mr]
+                    if self._dev_n is not None:
+                        self._dev_rank_map = step if self._dev_rank_map is None else step[self._dev_rank_map]
+        new_rank = np.fromiter((rank[m] for m in new_models), dtype=np.int32, count=len(new_models))
+        self._host["model_rank"] = self._grow("model_rank", mr, new_rank)
 
     def _free_device(self):
         """Give the device copy of the columns back (an insert makes it stale; without this every re-upload would leak the last one)."""
         ptrs, self._dev_ptrs = getattr(self, "_dev_ptrs", None), None
         self._dev = None
         self._dev_n = None
+        self._dev_rank_map = None
+        self._dev_cap = 0
         if ptrs and getattr(self.eng, "_h", None):
             self._free_ptrs(ptrs)
 
@@ -190,8 +259,33 @@ class UsageTable:
         self._free_device()
 
     def _upload(self):
+        """Bring the device copy up to date.  With one resident (device records [0, _dev_n) are host records [0, _dev_n)), the
+        host records past _dev_n, pending rows included, are appended to it (_append_on_device), growing the columns by
+        doubling when they are full; without one (a fresh table, or after load_columns) every column is uploaded."""
         if self._dev is not None:
             return
+        if self._dev_n is None:
+            self._upload_all()
+            return
+        self._materialise()
+        n_dev, n = self._dev_n, int(self._host["ts_us"].size)
+        rank_map = self._dev_rank_map
+        if n > n_dev or rank_map is not None:
+            cap = min(max(2 * self._dev_cap, n, 1024), APPEND_MAX) if n > self._dev_cap else None
+            try:
+                ptrs = self._append_on_device(n_dev, n - n_dev, rank_map, cap)
+            except BaseException:
+                self._free_device()               # (the next query uploads the table again: device ranks never disagree with the host)
+                raise
+            old, self._dev_ptrs = self._dev_ptrs, ptrs
+            if cap is not None:
+                self._dev_cap = cap
+                self._free_ptrs(old)
+            self._dev_n = n
+            self._dev_rank_map = None
+        self._dev = (n, self._dev_ptrs)
+
+    def _upload_all(self):
         self._free_device()
         self._materialise()
         n = int(self._host["ts_us"].size)
@@ -205,6 +299,31 @@ class UsageTable:
             ptrs[c] = p
         self._dev = (n, ptrs)
         self._dev_n = n
+        self._dev_cap = n
+
+    def _append_on_device(self, n: int, m: int, rank_map, cap) -> dict:
+        """host records [n, n + m) after the n resident ones (lgw_usage_append), the resident model ranks mapped through rank_map
+        (or None): in place when cap is None, else into fresh columns with room for cap records (the old ones stay as they
+        were, and on a failure the fresh ones are freed).  A new dict of the column pointers either way."""
+        lib, h = self._lib, self.eng._h
+        fresh = {}
+        try:
+            if cap is not None:
+                for c, d in zip(self.COLS, self.DTYPES):
+                    p = C.c_void_p()
+                    self.eng._ck(lib.lgw_device_alloc(h, max(cap * np.dtype(d).itemsize, 8), C.byref(p)), "device_alloc")
+                    fresh[c] = p
+            cols = (C.c_void_p * 8)(*[self._dev_ptrs[c].value for c in self.COLS])
+            grow = (C.c_void_p * 8)(*[fresh[c].value for c in self.COLS]) if cap is not None else None
+            new = [self._host[c][n:n + m] for c in self.COLS]
+            h_new = (C.c_void_p * 8)(*[a.ctypes.data for a in new])
+            rmap = np.ascontiguousarray(rank_map, np.int32) if rank_map is not None else None
+            self.eng._ck(lib.lgw_usage_append(h, cols, grow, n, h_new, m, rmap.ctypes.data_as(C.c_void_p) if rmap is not None else None,
+                                              rmap.size if rmap is not None else 0), "usage_append")
+        except BaseException:
+            self._free_ptrs(fresh)
+            raise
+        return fresh if cap is not None else dict(self._dev_ptrs)
 
     def __len__(self):
         return int(self._host["ts_us"].size) + len(self._pending_rows)
@@ -214,8 +333,10 @@ class UsageTable:
         self._materialise() if self._host.get("model_rank") is None or self._pending_rows else None
         ts = self._host["ts_us"]
         p = PERIODS[period]
-        lo = int(ts.min()) if ts.size else 0
-        hi = int(ts.max()) if ts.size else 0
+        rng = self._ts_range
+        if rng is None or rng[0] is not ts:
+            rng = self._ts_range = (ts, int(ts.min()) if ts.size else 0, int(ts.max()) if ts.size else 0)
+        lo, hi = rng[1], rng[2]
         if start is not None:
             lo = max(lo, to_us(start))
         if end is not None:
@@ -444,8 +565,10 @@ class UsageTable:
                 if self._dev is not None:
                     self._dev = (n_keep, fresh)
                 self._dev_n = n_keep
+                self._dev_cap = n_keep
         idx = np.flatnonzero(keep)                # (take() with indices is several times faster than a boolean mask here)
         self._host = {c: (a.take(idx) if a is not None else None) for c, a in h.items()}
+        self._ts_range = None
         self._ids = self._ids.take(idx)
         mask = keep.tolist()                      # (compress() over a list of bools, not over numpy bools: far faster)
         self._models = list(compress(self._models, mask))
@@ -476,6 +599,12 @@ class UsageTable:
         call and leaves it as it was)"""
         ms = C.c_float()
         self.eng._ck(self._lib.lgw_usage_retain_last_ms(self.eng._h, C.byref(ms)), "usage_retain_last_ms")
+        return ms.value
+
+    def append_last_ms(self) -> float:
+        """device time of the last lgw_usage_append (the copy of the new rows and k_usage_append), milliseconds"""
+        ms = C.c_float()
+        self.eng._ck(self._lib.lgw_usage_append_last_ms(self.eng._h, C.byref(ms)), "usage_append_last_ms")
         return ms.value
 
     def last_ms(self):
