@@ -279,6 +279,33 @@ int lgw_usage_append(lgw_engine* e, void* const d_cols[8], void* const d_grow[8]
 /* device time of the last lgw_usage_append (its copy and kernel), milliseconds (0 after a call that launched nothing) */
 int lgw_usage_append_last_ms(lgw_engine* e, float* ms);
 
+/* ---- loading the usage table from a `tokens_usage` SQLite file (tokens_usage_db.py:37-50) ------------------------------------
+ * Four calls, in order, on one engine (csrc/load.cuh):
+ * lgw_usage_load_decode: copies pages [1, n_pages] of h_file (page-locked host memory, n_bytes >= n_pages * page_size) to the
+ *   device in one copy, walks the table b-tree from page `root`, decodes every record and builds the model / provider
+ *   dictionaries.  out[6] = {LoadError (0: none; the rest of out is then meaningless), records, distinct model texts, distinct
+ *   provider texts, their total bytes (model, provider)}.  A page size that is not a power of two in [512, 65536], n_pages == 0
+ *   or too large for n_bytes, or n_bytes >= 2^33: LGW_ERR_ARG.  The file's own header is the caller's to check.
+ * lgw_usage_load_names: the distinct texts of `field` (0 model, 1 provider) in provisional-code order, read from h_file (the
+ *   buffer given to decode): buf holds out[4 + field] bytes, offs out[2 + field] + 1 offsets.
+ * lgw_usage_load_mark: maps (provisional code -> anything >= 0, or -1: refuse every record with that text) for both fields;
+ *   model_used[code] = 1 for each model text a kept record has; *n_keep = the records kept.
+ * lgw_usage_load_finish: the kept records in rowid order into d_cols (the eight UsageTable.COLS columns, n_keep records each,
+ *   caller-allocated) and into h_cols, with ids into h_ids, provider codes (prov_map[code], 0 for NULL) into h_prov; the ids of
+ *   the other records into h_refused.  model_map now gives ranks (0 for NULL); both maps must refuse what they refused in mark
+ *   (else LGW_ERR_ARG).  A call out of order: LGW_ERR_ARG.
+ * The load's device scratch (the file, per-record arrays, dictionaries) lives only from decode to the end of finish, or to a
+ * decode that found damage; lgw_usage_load_release frees it at any point (a load abandoned between the calls) and waits for
+ * the engine stream first.  A load is used once, at startup: nothing of it stays on the device but the caller's columns. */
+int lgw_usage_load_decode(lgw_engine* e, const uint8_t* h_file, uint64_t n_bytes, uint32_t page_size, uint32_t n_pages, uint32_t root, uint64_t out[6]);
+int lgw_usage_load_names(lgw_engine* e, const uint8_t* h_file, int field, uint8_t* buf, uint64_t* offs);
+int lgw_usage_load_mark(lgw_engine* e, const int32_t* model_map, const int32_t* prov_map, uint8_t* model_used, uint64_t* n_keep);
+int lgw_usage_load_finish(lgw_engine* e, const int32_t* model_map, const int32_t* prov_map, void* const d_cols[8], void* const h_cols[8],
+                          int64_t* h_ids, int32_t* h_prov, int64_t* h_refused);
+int lgw_usage_load_release(lgw_engine* e);
+/* device times of the last load, milliseconds: {host-to-device copy, b-tree walk and record decode, dictionaries, mark and finish} */
+int lgw_usage_load_last_ms(lgw_engine* e, float ms[4]);
+
 /* ---- request-body rewrite: SURVEY 8 rows a1, a3, a4 --------------------------------------------------
  * Replaces, for a batch of client requests, chat.py:31-45 (parse: lgw_bodies_scan) and, per upstream
  * attempt, chat.py:112-119,:135-139,:150,:164-168 (deepcopy + key assignments) followed by the encoder

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <string.h>
+#include <array>
 #include <string>
 #include <vector>
 
@@ -13,6 +14,7 @@
 #include "listing.cuh"
 #include "retain.cuh"
 #include "append.cuh"
+#include "load.cuh"
 #include "body_kernels.cuh"
 #include "doc_kernels.cuh"
 #include "transcript.cuh"
@@ -39,10 +41,10 @@ struct DevBuf {
     DevBuf(const DevBuf&) = delete;
     DevBuf& operator=(const DevBuf&) = delete;
     ~DevBuf() { if (p) cudaFree(p); }
+    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     cudaError_t reserve(size_t need, size_t slack = 0) {
         if (need <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr; cap = 0;
+        release();
         const cudaError_t r = cudaMalloc(&p, need + slack);
         if (r == cudaSuccess) cap = need + slack;
         return r;
@@ -130,6 +132,13 @@ struct lgw_engine {
         HostBuf host; DevBuf dev;
         cudaEvent_t ev[2]{}; float ms = 0;
     } append;
+    struct Load {                   // loading the usage table from a tokens_usage file (load.cuh); stage 1: decoded, 2: marked
+        DevBuf file, walk, recs, dict, maps, out;
+        DbGeom g{}; LoadRecs r{}; LoadDict d[2]{};
+        uint32_t n = 0, tiles = 0, n_names[2]{}; uint64_t n_keep = 0; int stage = 0;
+        std::vector<uint8_t> refused[2];        // the maps' refusals at mark time
+        cudaEvent_t ev[8]{}; float ms[4]{0, 0, 0, 0};
+    } load;
     struct Bodies {                 // request-body rewrite (rows a1-a4) and the document kernels, which share its input staging
         DevBuf plans, ops, blob; uint32_t n_plans = 0, n_ops = 0;       // the rule tables of lgw_rules_load
         DevBuf in, off, out_off, plan_idx, results, scans;      // per call: the packed bodies and five arrays indexed by body
@@ -866,6 +875,252 @@ extern "C" int lgw_usage_append(lgw_engine* e, void* const d_cols[8], void* cons
 extern "C" int lgw_usage_append_last_ms(lgw_engine* e, float* ms) {
     if (!e || !ms) return LGW_ERR_ARG;
     *ms = e->append.ms;
+    return LGW_OK;
+}
+
+// ---- loading the usage table from a tokens_usage file (tokens_usage_db.py:37-50) -----------------------------------------------
+// Consecutive 256-byte aligned pieces of one buffer: take(bytes) hands out the next one (base null: only counts).
+struct Carve {
+    uint8_t* base; size_t used = 0;
+    template <class T> T* take(size_t bytes) { T* p = (T*)(base ? base + used : nullptr); used += (bytes + 255) & ~(size_t)255; return p; }
+};
+
+// lgw_usage_load_finish's part of `out`: {ids, provider codes, refused ids, end}, after the tile offsets of k_load_mark; each
+// sized for all n records, so that mark reserves it once and finish never moves the offsets
+static std::array<size_t, 4> load_out_layout(uint32_t tiles, size_t n) {
+    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
+    const size_t o_ids = al(4ull * tiles + 16), o_prov = o_ids + al(8 * n), o_ref = o_prov + al(4 * n);
+    return {o_ids, o_prov, o_ref, o_ref + 8 * n + 8};
+}
+
+static void carve_recs(Carve& c, LoadRecs& r, size_t n) {
+    r.id = c.take<int64_t>(8 * n); r.ts = c.take<int64_t>(8 * n); r.cost = c.take<double>(8 * n);
+    for (int k = 0; k < 5; ++k) r.tok[k] = c.take<int32_t>(4 * n);
+    r.status = c.take<uint32_t>(4 * n); r.cell = c.take<CellRef>(sizeof(CellRef) * n);
+    for (int f = 0; f < 2; ++f) { r.text[f] = c.take<TextRef>(sizeof(TextRef) * n); r.slot[f] = c.take<uint32_t>(4 * n); }
+}
+
+extern "C" int lgw_usage_load_decode(lgw_engine* e, const uint8_t* h_file, uint64_t n_bytes, uint32_t page_size, uint32_t n_pages, uint32_t root, uint64_t out[6]) {
+    if (!e || !h_file || !out || page_size < 512 || page_size > 65536 || (page_size & (page_size - 1)) || n_pages == 0 ||
+        (uint64_t)n_pages * page_size > n_bytes || n_bytes >= (1ull << 33)) return LGW_ERR_ARG;
+    lgw_engine::Load& ld = e->load;
+    ld.stage = 0;
+    for (float& m : ld.ms) m = 0;
+    CK(e, cudaSetDevice(e->device));
+    const uint64_t bytes = (uint64_t)n_pages * page_size;
+    CK(e, ld.file.reserve(bytes));
+    if (!ld.ev[0]) CK(e, new_events(e, ld.ev, 8));
+    // walk scratch: two levels and their counts (n_pages + 1 each), the visited bitmap, then kinds / error / total / codes / bytes
+    const size_t lv = (size_t)n_pages + 1, words = n_pages / 32 + 1;
+    Carve wc{nullptr};
+    wc.take<uint32_t>(4 * lv); wc.take<uint32_t>(4 * lv); wc.take<uint32_t>(4 * lv); wc.take<uint32_t>(4 * words); wc.take<uint32_t>(64);
+    CK(e, ld.walk.reserve(wc.used));
+    Carve w{ld.walk.as<uint8_t>()};
+    uint32_t* level[2] = {w.take<uint32_t>(4 * lv), w.take<uint32_t>(4 * lv)};
+    uint32_t* cnt = w.take<uint32_t>(4 * lv);
+    uint32_t* visited = w.take<uint32_t>(4 * words);
+    uint32_t* ctr = w.take<uint32_t>(64);           // [0] kinds [1] error [2] total [3..4] codes, [6..9] name bytes (two u64)
+    CK(e, cudaEventRecord(ld.ev[0], e->stream));
+    CK(e, cudaMemcpyAsync(ld.file.p, h_file, bytes, cudaMemcpyHostToDevice, e->stream));
+    CK(e, cudaEventRecord(ld.ev[1], e->stream));
+    CK(e, cudaMemsetAsync(visited, 0, 4 * words, e->stream));
+    CK(e, cudaMemsetAsync(ctr, 0, 64, e->stream));
+    CK(e, cudaMemcpyAsync(level[0], &root, 4, cudaMemcpyHostToDevice, e->stream));
+    const DbGeom g{ld.file.as<uint8_t>(), page_size, n_pages};
+    ld.g = g;
+    uint32_t m = 1, cur = 0, err = 0, seen = 1, host_ctr[3] = {0, 0, 0};
+    for (uint32_t depth = 0;; ++depth) {           // one level a round; the host learns its kind and the next level's size
+        if (depth == LGW_LOAD_MAX_DEPTH) { err = LOAD_BAD_TREE; break; }
+        CK(e, cudaMemsetAsync(ctr, 0, 4, e->stream));
+        k_load_count<<<grid_for(e, m, 256, 8), 256, 0, e->stream>>>(g, level[cur], m, cnt, visited, ctr, ctr + 1);
+        k_list_scan<<<1, 1024, 0, e->stream>>>(cnt, m, ctr + 2);
+        e->launches += 2;
+        CK(e, cudaGetLastError());
+        CK(e, cudaMemcpyAsync(host_ctr, ctr, 12, cudaMemcpyDeviceToHost, e->stream));
+        CK(e, cudaStreamSynchronize(e->stream));
+        err = host_ctr[1];
+        if (err) break;
+        if (host_ctr[0] == 3) { err = LOAD_BAD_TREE; break; }
+        if (host_ctr[0] == 2) break;                 // the leaf level: cnt holds each leaf's first record
+        seen += host_ctr[2];
+        if (seen > n_pages) { err = LOAD_BAD_TREE; break; }
+        k_load_children<<<grid_for(e, m, 1, 64), 128, 0, e->stream>>>(g, level[cur], m, cnt, level[cur ^ 1], ctr + 1);
+        ++e->launches;
+        m = host_ctr[2];
+        cur ^= 1;
+    }
+    const uint32_t n = err ? 0 : host_ctr[2];
+    // records and dictionaries: a table of at least 2n slots a field
+    uint32_t cap = 64;
+    while (cap < 2ull * n) cap <<= 1;
+    Carve rc{nullptr};
+    LoadRecs r{};
+    carve_recs(rc, r, n);
+    CK(e, ld.recs.reserve(rc.used));
+    rc = Carve{ld.recs.as<uint8_t>()};
+    carve_recs(rc, r, n);
+    Carve dc{nullptr};
+    for (int f = 0; f < 2; ++f) { dc.take<uint64_t>(8ull * cap); dc.take<uint32_t>(4ull * cap); dc.take<NameRef>(sizeof(NameRef) * (size_t)(n ? n : 1)); }
+    CK(e, ld.dict.reserve(dc.used));
+    dc = Carve{ld.dict.as<uint8_t>()};
+    LoadDict d[2];
+    for (int f = 0; f < 2; ++f) {
+        d[f].table = dc.take<uint64_t>(8ull * cap); d[f].slot_code = dc.take<uint32_t>(4ull * cap);
+        d[f].names = dc.take<NameRef>(sizeof(NameRef) * (size_t)(n ? n : 1)); d[f].cap = cap;
+        d[f].n_codes = ctr + 3 + f; d[f].n_bytes = (unsigned long long*)(ctr + 6) + f;
+        CK(e, cudaMemsetAsync(d[f].table, 0, 8ull * cap, e->stream));
+    }
+    if (n) {
+        k_load_decode<<<grid_for(e, m, 1, 64), 128, 0, e->stream>>>(g, level[cur], m, cnt, r, ctr + 1);
+        ++e->launches;
+    }
+    CK(e, cudaEventRecord(ld.ev[2], e->stream));
+    if (n) {
+        k_load_dict<<<grid_for(e, n, 256, 8), 256, 0, e->stream>>>(g, r, n, d[0], d[1], ctr + 1);
+        ++e->launches;
+    }
+    CK(e, cudaEventRecord(ld.ev[3], e->stream));
+    CK(e, cudaGetLastError());
+    uint32_t res[10] = {};
+    CK(e, cudaMemcpyAsync(res, ctr, 40, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    read_ms(ld.ev[0], ld.ev[1], ld.ms[0]);
+    read_ms(ld.ev[1], ld.ev[2], ld.ms[1]);
+    read_ms(ld.ev[2], ld.ev[3], ld.ms[2]);
+    if (!err) err = res[1];
+    uint64_t nb[2];
+    memcpy(nb, res + 6, 16);
+    out[0] = err; out[1] = n; out[2] = res[3]; out[3] = res[4]; out[4] = nb[0]; out[5] = nb[1];
+    ld.r = r; ld.d[0] = d[0]; ld.d[1] = d[1];
+    ld.n = n; ld.n_names[0] = res[3]; ld.n_names[1] = res[4];
+    if (err) return lgw_usage_load_release(e);
+    ld.stage = 1;
+    return LGW_OK;
+}
+
+extern "C" int lgw_usage_load_names(lgw_engine* e, const uint8_t* h_file, int field, uint8_t* buf, uint64_t* offs) {
+    if (!e || !h_file || !offs || field < 0 || field > 1) return LGW_ERR_ARG;
+    lgw_engine::Load& ld = e->load;
+    if (ld.stage < 1) { e->err = "usage load: names before a decode"; return LGW_ERR_ARG; }
+    const uint32_t k = ld.n_names[field];
+    std::vector<NameRef> refs(k);
+    CK(e, cudaSetDevice(e->device));
+    if (k) CK(e, cudaMemcpyAsync(refs.data(), ld.d[field].names, k * sizeof(NameRef), cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    const DbGeom hg{h_file, ld.g.ps, ld.g.n_pages};
+    uint64_t at = 0;
+    for (uint32_t c = 0; c < k; ++c) {
+        offs[c] = at;
+        text_copy(hg, refs[c].cell, refs[c].t, buf + at);
+        at += refs[c].t.len;
+    }
+    offs[k] = at;
+    return LGW_OK;
+}
+
+// the two maps into the device staging; refusals recorded (mark) or checked against mark's (finish)
+static int load_maps(lgw_engine* e, const int32_t* model_map, const int32_t* prov_map, bool check, int32_t*& dm, int32_t*& dp) {
+    lgw_engine::Load& ld = e->load;
+    const int32_t* maps[2] = {model_map, prov_map};
+    for (int f = 0; f < 2; ++f) {
+        if (ld.n_names[f] && !maps[f]) return LGW_ERR_ARG;
+        std::vector<uint8_t> ref(ld.n_names[f]);
+        for (uint32_t c = 0; c < ld.n_names[f]; ++c) ref[c] = maps[f][c] < 0;
+        if (check && ref != ld.refused[f]) { e->err = "usage load: the maps refuse other texts than at mark"; return LGW_ERR_ARG; }
+        ld.refused[f] = std::move(ref);
+    }
+    const size_t n0 = ld.n_names[0], n1 = ld.n_names[1];
+    CK(e, ld.maps.reserve(4 * (n0 + n1) + n0 + 16));
+    dm = ld.maps.as<int32_t>();
+    dp = dm + n0;
+    if (n0) CK(e, cudaMemcpyAsync(dm, model_map, 4 * n0, cudaMemcpyHostToDevice, e->stream));
+    if (n1) CK(e, cudaMemcpyAsync(dp, prov_map, 4 * n1, cudaMemcpyHostToDevice, e->stream));
+    return LGW_OK;
+}
+
+extern "C" int lgw_usage_load_mark(lgw_engine* e, const int32_t* model_map, const int32_t* prov_map, uint8_t* model_used, uint64_t* n_keep) {
+    if (!e || !n_keep || (e->load.n_names[0] && !model_used)) return LGW_ERR_ARG;
+    lgw_engine::Load& ld = e->load;
+    if (ld.stage < 1) { e->err = "usage load: mark before a decode"; return LGW_ERR_ARG; }
+    CK(e, cudaSetDevice(e->device));
+    int32_t *dm, *dp;
+    TRY(load_maps(e, model_map, prov_map, false, dm, dp));
+    const uint32_t n = ld.n, tiles = (n + LGW_LOAD_TILE - 1) / LGW_LOAD_TILE;
+    uint8_t* used = (uint8_t*)(dp + ld.n_names[1]);
+    CK(e, ld.out.reserve(load_out_layout(tiles, n)[3]));
+    uint32_t* tile = ld.out.as<uint32_t>();
+    CK(e, cudaMemsetAsync(used, 0, ld.n_names[0] + 1, e->stream));
+    CK(e, cudaMemsetAsync(tile + tiles, 0, 4, e->stream));
+    CK(e, cudaEventRecord(ld.ev[4], e->stream));
+    if (tiles) {
+        k_load_mark<<<tiles, 1024, 0, e->stream>>>(ld.r, n, ld.d[0].slot_code, ld.d[1].slot_code, dm, dp, used, tile);
+        k_list_scan<<<1, 1024, 0, e->stream>>>(tile, tiles, tile + tiles);
+        e->launches += 2;
+    }
+    CK(e, cudaEventRecord(ld.ev[5], e->stream));
+    CK(e, cudaGetLastError());
+    uint32_t kept = 0;
+    CK(e, cudaMemcpyAsync(&kept, tile + tiles, 4, cudaMemcpyDeviceToHost, e->stream));
+    if (ld.n_names[0]) CK(e, cudaMemcpyAsync(model_used, used, ld.n_names[0], cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    ld.n_keep = *n_keep = kept;
+    ld.tiles = tiles;
+    ld.stage = 2;
+    return LGW_OK;
+}
+
+extern "C" int lgw_usage_load_finish(lgw_engine* e, const int32_t* model_map, const int32_t* prov_map, void* const d_cols[8], void* const h_cols[8],
+                                     int64_t* h_ids, int32_t* h_prov, int64_t* h_refused) {
+    if (!e) return LGW_ERR_ARG;
+    lgw_engine::Load& ld = e->load;
+    if (ld.stage != 2) { e->err = "usage load: finish before a mark"; return LGW_ERR_ARG; }
+    const uint64_t n = ld.n, k = ld.n_keep;
+    if (k && (!d_cols || !h_cols || !h_ids || !h_prov)) return LGW_ERR_ARG;
+    for (int c = 0; k && c < 8; ++c) if (!d_cols[c] || !h_cols[c]) return LGW_ERR_ARG;
+    if (n > k && !h_refused) return LGW_ERR_ARG;
+    CK(e, cudaSetDevice(e->device));
+    int32_t *dm, *dp;
+    TRY(load_maps(e, model_map, prov_map, true, dm, dp));
+    const std::array<size_t, 4> lay = load_out_layout(ld.tiles, ld.n);          // (mark sized `out` for all of it)
+    const size_t o_ids = lay[0], o_prov = lay[1], o_ref = lay[2];
+    uint8_t* ob = ld.out.as<uint8_t>();
+    LoadOut o{(int64_t*)(k ? d_cols[0] : nullptr), {}, (double*)(k ? d_cols[7] : nullptr), (int64_t*)(ob + o_ids), (int32_t*)(ob + o_prov), (int64_t*)(ob + o_ref)};
+    for (int c = 0; c < 6; ++c) o.i32[c] = (int32_t*)(k ? d_cols[1 + c] : nullptr);
+    CK(e, cudaEventRecord(ld.ev[6], e->stream));
+    if (ld.tiles) {
+        k_load_finish<<<ld.tiles, 1024, 0, e->stream>>>(ld.r, (uint32_t)n, ld.d[0].slot_code, ld.d[1].slot_code, dm, dp, ld.out.as<uint32_t>(), (uint32_t)k, o);
+        ++e->launches;
+    }
+    CK(e, cudaEventRecord(ld.ev[7], e->stream));
+    CK(e, cudaGetLastError());
+    static const size_t width[8] = {8, 4, 4, 4, 4, 4, 4, 8};
+    for (int c = 0; k && c < 8; ++c) CK(e, cudaMemcpyAsync(h_cols[c], d_cols[c], width[c] * k, cudaMemcpyDeviceToHost, e->stream));
+    if (k) CK(e, cudaMemcpyAsync(h_ids, o.id, 8 * k, cudaMemcpyDeviceToHost, e->stream));
+    if (k) CK(e, cudaMemcpyAsync(h_prov, o.prov, 4 * k, cudaMemcpyDeviceToHost, e->stream));
+    if (n > k) CK(e, cudaMemcpyAsync(h_refused, o.refused, 8 * (n - k), cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    float a = 0, b = 0;
+    read_ms(ld.ev[4], ld.ev[5], a);
+    read_ms(ld.ev[6], ld.ev[7], b);
+    ld.ms[3] = a + b;
+    return lgw_usage_load_release(e);
+}
+
+extern "C" int lgw_usage_load_release(lgw_engine* e) {
+    if (!e) return LGW_ERR_ARG;
+    lgw_engine::Load& ld = e->load;
+    CK(e, cudaSetDevice(e->device));
+    CK(e, cudaStreamSynchronize(e->stream));
+    for (DevBuf* b : {&ld.file, &ld.walk, &ld.recs, &ld.dict, &ld.maps, &ld.out}) b->release();
+    ld.stage = 0;
+    ld.n = ld.n_names[0] = ld.n_names[1] = 0;
+    ld.refused[0].clear(); ld.refused[1].clear();
+    return LGW_OK;
+}
+
+extern "C" int lgw_usage_load_last_ms(lgw_engine* e, float ms[4]) {
+    if (!e || !ms) return LGW_ERR_ARG;
+    for (int k = 0; k < 4; ++k) ms[k] = e->load.ms[k];
     return LGW_OK;
 }
 

@@ -5,6 +5,7 @@ llm_gateway_core/db/tokens_usage_db.py (TokensUsageDB) for rows a10/a11 of SURVE
   UsageTable.get_aggregated_usage()  <- TokensUsageDB.get_aggregated_usage  (:222-304)  [GPU kernel]
   UsageTable.get_latest_usage_records() <- TokensUsageDB.get_latest_usage_records (:69-117) [GPU kernel: page selection]
   UsageTable.cleanup_old_records()   <- TokensUsageDB.cleanup_old_records   (:164-198)  [GPU kernel: stable compaction]
+  UsageTable.load_tokens_usage_db()  <- the tokens_usage file itself        (:37-50)    [GPU kernels: SQLite pages decoded]
   stats_window(period, now)          <- llm_gateway_core/api/v1/stats.py:46-55
 
 Records live as SoA columns (40 B/record) in HBM; `model` is dictionary-encoded at ingest and
@@ -78,6 +79,111 @@ def sql_sum(costs: list[float]) -> float:
             return math.inf if exact > 0 else -math.inf
 
 
+class UsageDbNotModelled(Exception):
+    """A `tokens_usage` file or table the loader does not decode: WAL mode, a text encoding other than UTF-8, reserved bytes
+    per page, other payload fractions, another schema, or WITHOUT ROWID.  Nothing was loaded."""
+
+
+class UsageDbCorrupt(Exception):
+    """A structurally damaged `tokens_usage` file (see csrc/load.cuh LoadError).  Nothing was loaded."""
+
+
+# PRAGMA table_info(tokens_usage) of tokens_usage_db.py:37-50 (and gateway.SqliteUsageSink)
+TOKENS_USAGE_INFO = [(0, "id", "INTEGER", 0, None, 1), (1, "timestamp", "DATETIME", 1, None, 0)] + [
+    (k, c, "INTEGER", 0, "0", 0) for k, c in enumerate(("prompt_tokens", "completion_tokens", "total_tokens", "reasoning_tokens", "cached_tokens"), 2)] + [
+    (7, "cost", "REAL", 0, "0.0", 0), (8, "model", "TEXT", 0, None, 0), (9, "provider", "TEXT", 0, None, 0)]
+LOAD_ERRORS = {1: "a page number outside the file", 2: "a b-tree page of another type", 3: "a cell outside its page",
+               4: "a payload larger than the file or a broken overflow chain", 5: "a record header that does not fit its payload",
+               6: "a page reached twice, a level mixing interior and leaf pages, or a tree too deep",
+               8: "a rowid not above the one before it (duplicate or misordered cells)"}
+LOAD_ID_STORED = 7
+LOAD_MAX_BYTES = 1 << 33        # lgw_usage_load_decode takes files below this size
+
+
+def db_geometry(header: bytes, size: int):
+    """(page size, page count) of a SQLite file from its first 100 bytes and its size; UsageDbNotModelled for a file the
+    loader does not decode, UsageDbCorrupt for a header that is not SQLite's.  The page count is the header's when bytes
+    92-95 equal 24-27, else the file size's, and never more pages than the file holds."""
+    if len(header) < 100 or header[:16] != b"SQLite format 3\x00":
+        raise UsageDbCorrupt("not a SQLite 3 file")
+    ps = int.from_bytes(header[16:18], "big")
+    ps = 65536 if ps == 1 else ps
+    if ps < 512 or ps & (ps - 1):
+        raise UsageDbCorrupt(f"page size {ps}")
+    if header[18] == 2 or header[19] == 2:
+        raise UsageDbNotModelled("WAL-mode file")
+    if header[20] != 0:
+        raise UsageDbNotModelled(f"{header[20]} reserved bytes per page")
+    if tuple(header[21:24]) != (64, 32, 32):
+        raise UsageDbNotModelled(f"payload fractions {tuple(header[21:24])}")
+    if int.from_bytes(header[56:60], "big") != 1:
+        raise UsageDbNotModelled("text encoding other than UTF-8")
+    n_pages = int.from_bytes(header[28:32], "big") if header[92:96] == header[24:28] else size // ps
+    return ps, min(n_pages, size // ps)
+
+
+def read_tokens_usage_snapshot(db_path, alloc, free) -> dict:
+    """The bytes of a `tokens_usage` file as one consistent snapshot, with what the loader needs from SQLite itself.  Inside one
+    read transaction (BEGIN, then a SELECT on tokens_usage: SQLite rolls back a hot journal and takes a SHARED lock, and in
+    rollback-journal mode no writer can change the file while it is held) the schema row, PRAGMA table_info and
+    sqlite_sequence are read, and the file is read into alloc(size) (a uint8 array; given to free() if the call fails).  A file
+    the process may not write is opened read-only; SQLite then refuses to read it past a hot journal (UsageDbNotModelled).
+    Files of 2^33 bytes (8 GiB) or more are not decoded either."""
+    import os
+    import sqlite3
+    from urllib.parse import quote
+    if os.path.getsize(db_path) >= LOAD_MAX_BYTES:
+        raise UsageDbNotModelled(f"a file of {os.path.getsize(db_path)} bytes: the loader decodes files below 2^33 bytes")
+    mode = "rw" if os.access(db_path, os.W_OK) else "ro"
+    conn = sqlite3.connect(f"file:{quote(os.fspath(db_path))}?mode={mode}", uri=True, isolation_level=None)
+    try:
+        conn.execute("BEGIN")
+        try:
+            conn.execute("SELECT 1 FROM tokens_usage LIMIT 1").fetchall()
+        except sqlite3.OperationalError as e:                 # no such table, or a hot journal a read-only file cannot roll back
+            raise UsageDbNotModelled(str(e)) from None
+        except sqlite3.DatabaseError as e:                    # SQLite itself finds the file malformed
+            raise UsageDbCorrupt(str(e)) from None
+        row = conn.execute("SELECT rootpage FROM sqlite_schema WHERE type = 'table' AND name = 'tokens_usage'").fetchone()
+        if not row or not row[0]:
+            raise UsageDbNotModelled("tokens_usage is not a table (a view or a virtual table)")
+        root = row[0]
+        info = conn.execute("PRAGMA table_info(tokens_usage)").fetchall()
+        wr = conn.execute("SELECT wr FROM pragma_table_list WHERE schema = 'main' AND name = 'tokens_usage'").fetchone()
+        if info != TOKENS_USAGE_INFO or (wr and wr[0]):
+            raise UsageDbNotModelled("tokens_usage has another schema or is WITHOUT ROWID")
+        try:
+            seq = conn.execute("SELECT seq FROM sqlite_sequence WHERE name = 'tokens_usage'").fetchone()
+        except sqlite3.OperationalError:
+            seq = None
+        seq = seq or conn.execute("SELECT max(id) FROM tokens_usage").fetchone()
+        size = os.path.getsize(db_path)
+        buf = alloc(max(size, 100))
+        try:
+            with open(db_path, "rb") as f:
+                got = f.readinto(memoryview(buf)[:size])
+            ps, n_pages = db_geometry(bytes(buf[:min(got, 100)]), got)
+        except BaseException:
+            free(buf)
+            raise
+    finally:
+        conn.close()                      # (ends the read transaction)
+    return {"buf": buf, "size": got, "page_size": ps, "n_pages": n_pages, "root": int(root), "seq": int(seq[0] or 0)}
+
+
+def _utf8_or_none(b: bytes):
+    try:
+        return b.decode("utf-8")
+    except UnicodeDecodeError:
+        return None
+
+
+def _object_array(items: list) -> np.ndarray:
+    a = np.empty(len(items), dtype=object)
+    a[:] = items
+    return a
+
+
 def stats_window(period: str, now: datetime):
     """stats.py:46-55: (start_date, end_date) the stats endpoint asks for."""
     delta = {"hour": timedelta(hours=24), "day": timedelta(weeks=2), "week": timedelta(weeks=15), "month": timedelta(days=365)}[period]
@@ -105,6 +211,7 @@ class UsageTable:
     _dev_rank_map = None
     _dev_cap = 0
     _ts_range = None
+    rejected_ids = np.zeros(0, np.int64)      # ids of the records the last load_tokens_usage_db refused
 
     def __init__(self, engine):
         self.eng = engine
@@ -170,6 +277,120 @@ class UsageTable:
         self._rank = None
         self._dev_rank_map = None
         self._ts_range = None
+
+    def load_tokens_usage_db(self, db_path) -> int:
+        """Replace the table's contents with the records of the `tokens_usage` table of the SQLite file at db_path (as
+        tokens_usage_db.py and gateway.SqliteUsageSink write it), decoded on the device (csrc/load.cuh); the number loaded.
+        The table then equals one that got those records through insert_usage with their stored timestamps, in id order, and
+        was brought up to date on the device: same columns, model ranks, ids (gaps included), model and provider strings, and
+        the next id is sqlite_sequence's + 1.  The device columns are resident: the next query uploads nothing.
+        A record the table cannot hold is refused whole: its id goes to `rejected_ids` and the count to `rejected`.  It holds
+        a timestamp that is not TEXT exactly as datetime.isoformat() writes a naive datetime, a token count that is not an
+        INTEGER in [-2^31, 2^31) or NULL, a cost that is TEXT or BLOB, or a model or provider that is not NULL or valid UTF-8
+        TEXT.  Raises UsageDbNotModelled or UsageDbCorrupt (or the engine's error) and leaves the table as it was."""
+        snap = read_tokens_usage_snapshot(db_path, self._load_alloc, self._load_free)
+        try:
+            got = self._load_records(snap)
+        finally:
+            self._load_free(snap["buf"])
+        cols, ids, names, prov_names, prov, refused, dev = got
+        n = int(ids.size)
+        old = getattr(self, "_dev_ptrs", None)
+        self._host = cols
+        self._ids = ids
+        self._seq = snap["seq"]
+        self._names = [None] + names
+        self._rank = {m: i for i, m in enumerate(self._names)}
+        self._models = _object_array(self._names).take(cols["model_rank"]).tolist()
+        self._providers = _object_array([None] + prov_names).take(prov).tolist()
+        self._pending_rows = []
+        self._fixed_names = None
+        self._hbuf = None
+        self._ts_range = None
+        self._dev_rank_map = None
+        self._dev_ptrs = dev
+        self._dev = (n, dev)
+        self._dev_n = self._dev_cap = n
+        if old:
+            self._free_ptrs(old)
+        self.rejected += int(refused.size)
+        self.rejected_ids = refused
+        return n
+
+    def _load_records(self, snap: dict):
+        """csrc/load.cuh over the snapshot's bytes: (host columns, ids, ranked model names, provider names, provider codes,
+        refused ids, device columns).  Distinct texts come back once each; a text that is not valid UTF-8 refuses its records."""
+        try:
+            return self._load_steps(snap)
+        finally:
+            self._load_call("release")                # (the load's device scratch is only needed until finish)
+
+    def _load_steps(self, snap: dict):
+        buf = snap["buf"]
+        bp = buf.ctypes.data_as(C.c_void_p)
+        out = np.zeros(6, np.uint64)
+        self._load_call("decode", bp, snap["size"], snap["page_size"], snap["n_pages"], snap["root"], out.ctypes.data_as(C.c_void_p))
+        err, n, counts, nbytes = int(out[0]), int(out[1]), (int(out[2]), int(out[3])), (int(out[4]), int(out[5]))
+        if err == LOAD_ID_STORED:
+            raise UsageDbNotModelled("tokens_usage stores its id column: id is not a rowid alias")
+        if err:
+            raise UsageDbCorrupt(LOAD_ERRORS.get(err, f"load error {err}"))
+        texts = []
+        for field in (0, 1):
+            raw = np.zeros(max(nbytes[field], 1), np.uint8)
+            offs = np.zeros(counts[field] + 1, np.uint64)
+            self._load_call("names", bp, field, raw.ctypes.data_as(C.c_void_p), offs.ctypes.data_as(C.c_void_p))
+            blob, o = raw.tobytes(), offs.tolist()
+            texts.append([_utf8_or_none(blob[o[k]:o[k + 1]]) for k in range(counts[field])])
+        mm = np.array([0 if t is not None else -1 for t in texts[0]] or [0], np.int32)
+        pm = np.array([k + 1 if t is not None else -1 for k, t in enumerate(texts[1])] or [0], np.int32)
+        used = np.zeros(max(counts[0], 1), np.uint8)
+        n_keep = C.c_uint64(0)
+        self._load_call("mark", mm.ctypes.data_as(C.c_void_p), pm.ctypes.data_as(C.c_void_p), used.ctypes.data_as(C.c_void_p), C.byref(n_keep))
+        k = n_keep.value
+        names = sorted({texts[0][c] for c in np.flatnonzero(used[:counts[0]]).tolist()}, key=lambda s: s.encode("utf-8"))
+        rank = {m: i + 1 for i, m in enumerate(names)}
+        mm = np.array([rank.get(t, 0) if t is not None else -1 for t in texts[0]] or [0], np.int32)
+        cols = {c: np.empty(k, d) for c, d in zip(self.COLS, self.DTYPES)}
+        ids, prov, refused = np.empty(k, np.int64), np.empty(k, np.int32), np.empty(n - k, np.int64)
+        dev = self._load_cols_alloc(k)
+        try:
+            d_cols = (C.c_void_p * 8)(*[dev[c].value if dev else None for c in self.COLS])
+            h_cols = (C.c_void_p * 8)(*[cols[c].ctypes.data for c in self.COLS])
+            self._load_call("finish", mm.ctypes.data_as(C.c_void_p), pm.ctypes.data_as(C.c_void_p), d_cols, h_cols,
+                            ids.ctypes.data_as(C.c_void_p), prov.ctypes.data_as(C.c_void_p), refused.ctypes.data_as(C.c_void_p))
+        except BaseException:
+            self._free_ptrs(dev)
+            raise
+        return cols, ids, names, texts[1], prov, refused, dev
+
+    # the loader's seams: a CPU stand-in replaces these with the host build of csrc/load.cuh and numpy buffers
+    def _load_call(self, step: str, *args):
+        self.eng._ck(getattr(self._lib, "lgw_usage_load_" + step)(self.eng._h, *args), "usage_load_" + step)
+
+    def _load_alloc(self, nbytes: int) -> np.ndarray:
+        return self.eng.alloc_pinned(nbytes)
+
+    def _load_free(self, buf: np.ndarray):
+        self._lib.lgw_free_pinned(self.eng._h, C.c_void_p(buf.ctypes.data))
+
+    def _load_cols_alloc(self, n: int) -> dict:
+        ptrs = {}
+        try:
+            for c, d in zip(self.COLS, self.DTYPES):
+                p = C.c_void_p()
+                self.eng._ck(self._lib.lgw_device_alloc(self.eng._h, max(n * np.dtype(d).itemsize, 8), C.byref(p)), "device_alloc")
+                ptrs[c] = p
+        except BaseException:
+            self._free_ptrs(ptrs)
+            raise
+        return ptrs
+
+    def load_last_ms(self) -> dict:
+        """device times of the last load_tokens_usage_db, milliseconds"""
+        ms = (C.c_float * 4)()
+        self.eng._ck(self._lib.lgw_usage_load_last_ms(self.eng._h, C.byref(ms)), "usage_load_last_ms")
+        return {"copy": ms[0], "decode": ms[1], "dictionary": ms[2], "compaction": ms[3]}
 
     def _grow(self, key: str, a: np.ndarray, new: np.ndarray) -> np.ndarray:
         """a followed by new, as an exact-length view of a buffer of this table with room to grow (doubling): when a is the
