@@ -306,6 +306,31 @@ int lgw_usage_load_release(lgw_engine* e);
 /* device times of the last load, milliseconds: {host-to-device copy, b-tree walk and record decode, dictionaries, mark and finish} */
 int lgw_usage_load_last_ms(lgw_engine* e, float ms[4]);
 
+/* ---- saving the usage table as a `tokens_usage` SQLite file (the file lgw_usage_load_* reads) --------------------------------
+ * Two calls, in order, on one engine (csrc/save.cuh):
+ * lgw_usage_save_plan: the n records of d_cols (the eight UsageTable.COLS device columns, ts_us 16-byte aligned) with their ids
+ *   (h_ids, ascending) and provider codes (h_prov), host memory copied up for the call.  Text tables: text k of `models` is
+ *   model rank k, of `providers` provider code k; len[k] is its byte count, LGW_SAVE_TEXT_NULL for NULL or LGW_SAVE_TEXT_BAD
+ *   for a text the file cannot hold; off has n + 1 entries, off[n] the blob's size.  A record is kept unless a text of it is
+ *   BAD or its ts_us has no datetime.isoformat() text (years 0001-9999).  Lays out the file for page_size (a power of two in
+ *   [1024, 65536]): out[5] = {pages of the whole file, table root page, index root page, kept records, refused records}.
+ *   Pages 1 (header and sqlite_schema) and 2 (sqlite_sequence) are the caller's.  LGW_ERR_ARG: n >= 2^32, a null pointer the
+ *   call needs, a misaligned ts_us column, an empty text table, a rank or code outside its table, ids not ascending, or a
+ *   file of 2^32 - 1 pages or more.
+ * lgw_usage_save_write: pages 3 .. out[0] into h_file + 2 * page_size (page-locked, out[0] * page_size bytes), the refused
+ *   records' ids in record order into h_refused (out[4] entries).
+ * The save's device scratch (ids and codes, per-record arrays, the page pool, the file image) lives only from plan to the end
+ * of write; lgw_usage_save_release frees it at any point and waits for the engine stream first. */
+typedef struct lgw_save_text { const uint8_t* blob; const uint64_t* off; const uint32_t* len; uint32_t n, pad; } lgw_save_text;
+#define LGW_SAVE_TEXT_NULL 0xFFFFFFFFu
+#define LGW_SAVE_TEXT_BAD 0xFFFFFFFEu
+int lgw_usage_save_plan(lgw_engine* e, void* const d_cols[8], uint64_t n, const int64_t* h_ids, const int32_t* h_prov,
+                        const lgw_save_text* models, const lgw_save_text* providers, uint32_t page_size, uint64_t out[5]);
+int lgw_usage_save_write(lgw_engine* e, uint8_t* h_file, int64_t* h_refused);
+int lgw_usage_save_release(lgw_engine* e);
+/* device times of the last save, milliseconds: {ids and codes up, keep, sort, pack, page writes, download} */
+int lgw_usage_save_last_ms(lgw_engine* e, float ms[6]);
+
 /* ---- request-body rewrite: SURVEY 8 rows a1, a3, a4 --------------------------------------------------
  * Replaces, for a batch of client requests, chat.py:31-45 (parse: lgw_bodies_scan) and, per upstream
  * attempt, chat.py:112-119,:135-139,:150,:164-168 (deepcopy + key assignments) followed by the encoder

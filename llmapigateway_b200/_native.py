@@ -20,7 +20,8 @@ EXPORTS = [
     "lgw_usage_rollup_accum", "lgw_usage_rollup_emit", "lgw_rollup_bucket_of", "lgw_rollup_buckets_of", "lgw_rollup_last_ms",
     "lgw_usage_latest", "lgw_usage_latest_last_ms", "lgw_usage_retain", "lgw_usage_retain_last_ms",
     "lgw_usage_append", "lgw_usage_append_last_ms", "lgw_usage_load_decode", "lgw_usage_load_names", "lgw_usage_load_mark",
-    "lgw_usage_load_finish", "lgw_usage_load_release", "lgw_usage_load_last_ms", "lgw_device_alloc", "lgw_device_free", "lgw_device_upload", "lgw_device_download", "lgw_device_zero",
+    "lgw_usage_load_finish", "lgw_usage_load_release", "lgw_usage_load_last_ms",
+    "lgw_usage_save_plan", "lgw_usage_save_write", "lgw_usage_save_release", "lgw_usage_save_last_ms", "lgw_device_alloc", "lgw_device_free", "lgw_device_upload", "lgw_device_download", "lgw_device_zero",
     "lgw_transcripts_enable", "lgw_step_transcript_run", "lgw_step_transcript_fetch", "lgw_transcript_last_ms",
     "lgw_documents_usage", "lgw_rules_load", "lgw_bodies_scan", "lgw_bodies_rewrite", "lgw_bodies_rewrite_device", "lgw_bodies_last_ms",
     "lgw_documents_text", "lgw_documents_text_last_ms",
@@ -90,6 +91,11 @@ def load():
                                           C.c_void_p, C.c_void_p, C.c_void_p]
     lib.lgw_usage_load_release.argtypes = [C.c_void_p]
     lib.lgw_usage_load_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
+    lib.lgw_usage_save_plan.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_uint32, C.c_void_p]
+    lib.lgw_usage_save_write.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.lgw_usage_save_release.argtypes = [C.c_void_p]
+    lib.lgw_usage_save_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 6)]
     lib.lgw_device_alloc.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p)]
     lib.lgw_device_free.argtypes = [C.c_void_p, C.c_void_p]
     lib.lgw_device_upload.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]

@@ -15,6 +15,7 @@
 #include "retain.cuh"
 #include "append.cuh"
 #include "load.cuh"
+#include "save.cuh"
 #include "body_kernels.cuh"
 #include "doc_kernels.cuh"
 #include "transcript.cuh"
@@ -29,6 +30,7 @@ static_assert(sizeof(SegResult) == sizeof(lgw_seg_result), "lgw_seg_result layou
 static_assert(sizeof(RollupRow) == sizeof(lgw_rollup_row), "lgw_rollup_row layout");
 static_assert(sizeof(DocUsage) == sizeof(lgw_doc_usage), "lgw_doc_usage layout");
 static_assert(sizeof(TextMark) == sizeof(lgw_text_mark), "lgw_text_mark layout");
+static_assert(sizeof(SaveText) == sizeof(lgw_save_text), "lgw_save_text layout");
 
 static thread_local std::string g_create_error;
 
@@ -139,6 +141,11 @@ struct lgw_engine {
         std::vector<uint8_t> refused[2];        // the maps' refusals at mark time
         cudaEvent_t ev[8]{}; float ms[4]{0, 0, 0, 0};
     } load;
+    struct Save {                   // saving the usage table as a tokens_usage file (save.cuh); stage 1: planned
+        DevBuf in, recs, sort, pack, pool, img;
+        SaveCtx c{}; uint32_t n = 0, kept = 0, n_pool = 0, n_ovfl = 0, pages = 0; int64_t* refused = nullptr; int stage = 0;
+        cudaEvent_t ev[8]{}; float ms[6]{0, 0, 0, 0, 0, 0};
+    } save;
     struct Bodies {                 // request-body rewrite (rows a1-a4) and the document kernels, which share its input staging
         DevBuf plans, ops, blob; uint32_t n_plans = 0, n_ops = 0;       // the rule tables of lgw_rules_load
         DevBuf in, off, out_off, plan_idx, results, scans;      // per call: the packed bodies and five arrays indexed by body
@@ -1121,6 +1128,218 @@ extern "C" int lgw_usage_load_release(lgw_engine* e) {
 extern "C" int lgw_usage_load_last_ms(lgw_engine* e, float ms[4]) {
     if (!e || !ms) return LGW_ERR_ARG;
     for (int k = 0; k < 4; ++k) ms[k] = e->load.ms[k];
+    return LGW_OK;
+}
+
+// ---- saving the usage table as a tokens_usage file (save.cuh) ---------------------------------------------------------------
+extern "C" int lgw_usage_save_plan(lgw_engine* e, void* const d_cols[8], uint64_t n, const int64_t* h_ids, const int32_t* h_prov,
+                                   const lgw_save_text* models, const lgw_save_text* providers, uint32_t page_size, uint64_t out[5]) {
+    if (!e || !out || !models || !providers || n >= (1ull << 32) || page_size < 1024 || page_size > 65536 || (page_size & (page_size - 1))) return LGW_ERR_ARG;
+    if (n && (!d_cols || !h_ids || !h_prov)) return LGW_ERR_ARG;
+    for (int c = 0; n && c < 8; ++c) if (!d_cols[c]) return LGW_ERR_ARG;
+    if (n && ((uintptr_t)d_cols[0] & 15)) return LGW_ERR_ARG;
+    const lgw_save_text* tx[2] = {models, providers};
+    uint64_t blob[2];
+    for (int f = 0; f < 2; ++f) {
+        if (!tx[f]->n || !tx[f]->off || !tx[f]->len) return LGW_ERR_ARG;
+        blob[f] = tx[f]->off[tx[f]->n];
+        if (blob[f] && !tx[f]->blob) return LGW_ERR_ARG;
+    }
+    TRY(lgw_usage_save_release(e));
+    lgw_engine::Save& sv = e->save;
+    for (float& m : sv.ms) m = 0;
+    if (!sv.ev[0]) CK(e, new_events(e, sv.ev, 8));
+    const uint32_t N = (uint32_t)n, U = page_size, M = N ? N : 1;
+    const uint32_t ktiles = (N + LGW_LOAD_TILE - 1) / LGW_LOAD_TILE;
+    // inputs: ids, provider codes, the two text tables
+    auto carve_in = [&](Carve& c, int64_t*& ids, int32_t*& prov, SaveText* t) {
+        ids = c.take<int64_t>(8ull * N); prov = c.take<int32_t>(4ull * N);
+        for (int f = 0; f < 2; ++f) {
+            t[f].off = c.take<uint64_t>(8ull * (tx[f]->n + 1)); t[f].len = c.take<uint32_t>(4ull * tx[f]->n);
+            t[f].blob = c.take<uint8_t>(blob[f]); t[f].n = tx[f]->n; t[f].pad = 0;
+        }
+    };
+    int64_t* ids; int32_t* prov; SaveText t[2];
+    Carve ic{nullptr};
+    carve_in(ic, ids, prov, t);
+    CK(e, sv.in.reserve(ic.used));
+    ic = Carve{sv.in.as<uint8_t>()};
+    carve_in(ic, ids, prov, t);
+    // per record: kept record, table cell size, overflow pages, two sort keys and indices, refused ids; keep tiles; counters
+    auto carve_recs = [&](Carve& c, uint32_t*& kidx, uint32_t*& lsz, uint32_t*& lov, uint64_t** key, uint32_t** idx, int64_t*& ref,
+                          uint32_t*& tiles, unsigned long long*& ctr) {
+        kidx = c.take<uint32_t>(4ull * M); lsz = c.take<uint32_t>(4ull * M); lov = c.take<uint32_t>(4ull * M);
+        key[0] = c.take<uint64_t>(8ull * M); key[1] = c.take<uint64_t>(8ull * M);
+        idx[0] = c.take<uint32_t>(4ull * M); idx[1] = c.take<uint32_t>(4ull * M);
+        ref = c.take<int64_t>(8ull * M); tiles = c.take<uint32_t>(4ull * (ktiles + 1)); ctr = c.take<unsigned long long>(32);
+    };
+    uint32_t *kidx, *lsz, *lov, *idx[2], *tcount; uint64_t* key[2]; int64_t* refused; unsigned long long* ctr;
+    Carve rc{nullptr};
+    carve_recs(rc, kidx, lsz, lov, key, idx, refused, tcount, ctr);
+    CK(e, sv.recs.reserve(rc.used));
+    rc = Carve{sv.recs.as<uint8_t>()};
+    carve_recs(rc, kidx, lsz, lov, key, idx, refused, tcount, ctr);
+    CK(e, cudaSetDevice(e->device));
+    CK(e, cudaEventRecord(sv.ev[0], e->stream));
+    if (N) CK(e, cudaMemcpyAsync(ids, h_ids, 8ull * N, cudaMemcpyHostToDevice, e->stream));
+    if (N) CK(e, cudaMemcpyAsync(prov, h_prov, 4ull * N, cudaMemcpyHostToDevice, e->stream));
+    for (int f = 0; f < 2; ++f) {
+        CK(e, cudaMemcpyAsync((void*)t[f].off, tx[f]->off, 8ull * (tx[f]->n + 1), cudaMemcpyHostToDevice, e->stream));
+        CK(e, cudaMemcpyAsync((void*)t[f].len, tx[f]->len, 4ull * tx[f]->n, cudaMemcpyHostToDevice, e->stream));
+        if (blob[f]) CK(e, cudaMemcpyAsync((void*)t[f].blob, tx[f]->blob, blob[f], cudaMemcpyHostToDevice, e->stream));
+    }
+    CK(e, cudaEventRecord(sv.ev[1], e->stream));
+    // 1. keep
+    SaveIn in{};
+    if (N) {
+        in.ts = (const int64_t*)d_cols[0]; in.cost = (const double*)d_cols[7];
+        for (int c = 0; c < 6; ++c) in.i32[c] = (const int32_t*)d_cols[1 + c];
+    }
+    in.id = ids; in.prov = prov; in.text[0] = t[0]; in.text[1] = t[1];
+    CK(e, cudaMemsetAsync(ctr, 0xFF, 8, e->stream));
+    CK(e, cudaMemsetAsync(ctr + 1, 0, 24, e->stream));
+    CK(e, cudaMemsetAsync(tcount + ktiles, 0, 4, e->stream));
+    if (ktiles) {
+        k_save_count<<<ktiles, 1024, 0, e->stream>>>(in, N, tcount, ctr, ctr + 1, (uint32_t*)(ctr + 2));
+        k_list_scan<<<1, 1024, 0, e->stream>>>(tcount, ktiles, tcount + ktiles);
+        e->launches += 2;
+    }
+    CK(e, cudaGetLastError());
+    unsigned long long res[3];
+    uint32_t K = 0;
+    CK(e, cudaMemcpyAsync(res, ctr, 24, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(&K, tcount + ktiles, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    if (res[2] & 2) { e->err = "usage save: a model rank or provider code outside its text table"; lgw_usage_save_release(e); return LGW_ERR_ARG; }
+    if (res[2] & 1) { e->err = "usage save: ids not ascending in record order"; lgw_usage_save_release(e); return LGW_ERR_ARG; }
+    if (ktiles) {
+        k_save_keep<<<ktiles, 1024, 0, e->stream>>>(in, N, U, tcount, ctr, kidx, lsz, lov, key[0], idx[0], refused);
+        ++e->launches;
+    }
+    CK(e, cudaEventRecord(sv.ev[2], e->stream));
+    // 2. sort: the stable LSD passes over the digits the key range needs
+    const uint64_t range = K ? res[1] - res[0] : 0;
+    int bits = 0;
+    while (bits < 64 && (range >> bits)) ++bits;
+    const int passes = (bits + 7) / 8;
+    const uint32_t stiles = (K + LGW_LIST_STILE - 1) / LGW_LIST_STILE;
+    uint32_t cur = 0;
+    if (passes && K > 1) {
+        CK(e, sv.sort.reserve((256ull * stiles + 256) * 4));
+        uint32_t* hist = sv.sort.as<uint32_t>();
+        uint32_t* totals = hist + 256ull * stiles;
+        for (int p = 0; p < passes; ++p) {
+            k_lsd_hist<<<stiles, 256, 0, e->stream>>>(key[cur], K, 8 * p, hist, stiles);
+            k_list_scan<<<256, 1024, 0, e->stream>>>(hist, stiles, totals);
+            k_lsd_scatter<<<stiles, 256, 0, e->stream>>>(key[cur], idx[cur], K, 8 * p, hist, totals, stiles, key[cur ^ 1], idx[cur ^ 1]);
+            e->launches += 3;
+            cur ^= 1;
+        }
+    }
+    CK(e, cudaEventRecord(sv.ev[3], e->stream));
+    // 3. pack, level by level; the pool holds at most twice each tree's leaves (every interior page has two children or more)
+    const uint32_t tile = save_tile(U), ptiles = pack_tiles(K, tile), pool_cap = 4 * M + 4 * LGW_SAVE_MAX_LEVELS;
+    Carve pc{nullptr};
+    for (int k = 0; k < 4; ++k) pc.take<uint32_t>(4ull * M);
+    pc.take<uint32_t>(4ull * (ptiles + 1)); pc.take<uint32_t>(4ull * (ptiles + 1));
+    CK(e, sv.pack.reserve(pc.used));
+    pc = Carve{sv.pack.as<uint8_t>()};
+    uint32_t *pstart = pc.take<uint32_t>(4ull * M), *pcnt = pc.take<uint32_t>(4ull * M), *isz_a = pc.take<uint32_t>(4ull * M), *isz_b = pc.take<uint32_t>(4ull * M);
+    uint32_t *tpages = pc.take<uint32_t>(4ull * (ptiles + 1)), *tovfl = pc.take<uint32_t>(4ull * (ptiles + 1));
+    CK(e, sv.pool.reserve((size_t)pool_cap * sizeof(PageDesc)));
+    SaveCtx c{};
+    c.in = in; c.U = U; c.kidx = kidx; c.sidx = idx[cur]; c.lsz = lsz; c.lov = lov; c.pool = sv.pool.as<PageDesc>(); c.lock = (1u << 30) / U + 1;
+    uint32_t used = 0, n_ovfl = 0;
+    for (uint32_t tree = 0; tree < 2; ++tree) {
+        const uint32_t* isz = lsz;
+        uint32_t* next = isz_a;
+        if (tree == 1) {
+            if (K) k_save_entry_sizes<<<grid_for(e, K, 256, 8), 256, 0, e->stream>>>(in, kidx, c.sidx, K, isz_a);
+            isz = isz_a; next = isz_b;
+        }
+        uint32_t m = K, kind = tree ? SAVE_INDEX_LEAF : SAVE_TABLE_LEAF;
+        for (uint32_t level = 0;; ++level) {
+            if (level == LGW_SAVE_MAX_LEVELS) { e->err = "usage save: b-tree deeper than LGW_SAVE_MAX_LEVELS"; lgw_usage_save_release(e); return LGW_ERR_CAPACITY; }
+            const uint32_t tiles = pack_tiles(m, tile);
+            const bool ovfl = tree == 0 && level == 0;
+            k_save_pack<<<(tiles + 127) / 128, 128, 0, e->stream>>>(isz, m, tiles, kind, U, pstart, pcnt, tpages, ovfl ? lov : nullptr, tovfl);
+            k_list_scan<<<1, 1024, 0, e->stream>>>(tpages, tiles, tpages + tiles);
+            if (ovfl) k_list_scan<<<1, 1024, 0, e->stream>>>(tovfl, tiles, tovfl + tiles);
+            e->launches += 2 + ovfl;
+            CK(e, cudaGetLastError());
+            uint32_t P = 0;
+            CK(e, cudaMemcpyAsync(&P, tpages + tiles, 4, cudaMemcpyDeviceToHost, e->stream));
+            if (ovfl) CK(e, cudaMemcpyAsync(&n_ovfl, tovfl + tiles, 4, cudaMemcpyDeviceToHost, e->stream));
+            CK(e, cudaStreamSynchronize(e->stream));
+            if ((uint64_t)used + P > pool_cap) { e->err = "usage save: page pool overflow"; lgw_usage_save_release(e); return LGW_ERR_CUDA; }
+            c.base[tree][level] = used;
+            k_save_gather<<<grid_for(e, tiles, 1, 64), 128, 0, e->stream>>>(c, tree, level, m, tiles, tpages, pstart, pcnt, sv.pool.as<PageDesc>(), used, next);
+            ++e->launches;
+            used += P;
+            if (P == 1) { c.levels[tree] = level + 1; c.base[tree][level + 1] = used; break; }
+            m = tree ? P - 1 : P;
+            kind = tree ? SAVE_INDEX_INTERIOR : SAVE_TABLE_INTERIOR;
+            isz = next;
+            next = next == isz_a ? isz_b : isz_a;
+        }
+    }
+    const uint64_t laid = 2ull + used + n_ovfl, pages = laid + (laid >= c.lock);      // (the lock-byte page, unused)
+    if (pages > 0xFFFFFFFEull) { e->err = "usage save: more pages than a SQLite file holds"; lgw_usage_save_release(e); return LGW_ERR_ARG; }
+    if (K) k_save_ovfl_abs<<<grid_for(e, K, 256, 8), 256, 0, e->stream>>>(lov, K, ptiles, tile, tovfl, LGW_SAVE_POOL0 + used);
+    CK(e, cudaEventRecord(sv.ev[4], e->stream));
+    CK(e, cudaGetLastError());
+    CK(e, cudaStreamSynchronize(e->stream));
+    read_ms(sv.ev[0], sv.ev[1], sv.ms[0]);
+    read_ms(sv.ev[1], sv.ev[2], sv.ms[1]);
+    read_ms(sv.ev[2], sv.ev[3], sv.ms[2]);
+    read_ms(sv.ev[3], sv.ev[4], sv.ms[3]);
+    sv.c = c; sv.n = N; sv.kept = K; sv.n_pool = used; sv.n_ovfl = n_ovfl; sv.pages = (uint32_t)pages; sv.refused = refused; sv.stage = 1;
+    out[0] = pages; out[1] = save_page(c, LGW_SAVE_POOL0 + c.base[0][c.levels[0] - 1]); out[2] = save_page(c, LGW_SAVE_POOL0 + c.base[1][c.levels[1] - 1]);
+    out[3] = K; out[4] = N - K;
+    return LGW_OK;
+}
+
+extern "C" int lgw_usage_save_write(lgw_engine* e, uint8_t* h_file, int64_t* h_refused) {
+    if (!e) return LGW_ERR_ARG;
+    lgw_engine::Save& sv = e->save;
+    if (sv.stage != 1) { e->err = "usage save: write before a plan"; return LGW_ERR_ARG; }
+    if (!h_file || (sv.n > sv.kept && !h_refused)) return LGW_ERR_ARG;
+    CK(e, cudaSetDevice(e->device));
+    const uint32_t U = sv.c.U;
+    const uint64_t bytes = (uint64_t)(sv.pages - 2) * U;
+    CK(e, sv.img.reserve(bytes));
+    if (sv.pages > sv.c.lock) CK(e, cudaMemsetAsync(sv.img.as<uint8_t>() + (uint64_t)(sv.c.lock - LGW_SAVE_POOL0) * U, 0, U, e->stream));
+    CK(e, cudaFuncSetAttribute(k_save_pages, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)U));
+    CK(e, cudaEventRecord(sv.ev[5], e->stream));
+    k_save_pages<<<grid_for(e, sv.n_pool, 1, 16), 128, U, e->stream>>>(sv.c, sv.n_pool, sv.img.as<uint8_t>());
+    ++e->launches;
+    if (sv.n_ovfl) { k_save_chains<<<grid_for(e, sv.kept, 256, 8), 256, 0, e->stream>>>(sv.c, sv.kept, sv.img.as<uint8_t>()); ++e->launches; }
+    CK(e, cudaEventRecord(sv.ev[6], e->stream));
+    CK(e, cudaGetLastError());
+    CK(e, cudaMemcpyAsync(h_file + 2ull * U, sv.img.p, bytes, cudaMemcpyDeviceToHost, e->stream));
+    if (sv.n > sv.kept) CK(e, cudaMemcpyAsync(h_refused, sv.refused, 8ull * (sv.n - sv.kept), cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaEventRecord(sv.ev[7], e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    read_ms(sv.ev[5], sv.ev[6], sv.ms[4]);
+    read_ms(sv.ev[6], sv.ev[7], sv.ms[5]);
+    return lgw_usage_save_release(e);
+}
+
+extern "C" int lgw_usage_save_release(lgw_engine* e) {
+    if (!e) return LGW_ERR_ARG;
+    lgw_engine::Save& sv = e->save;
+    CK(e, cudaSetDevice(e->device));
+    CK(e, cudaStreamSynchronize(e->stream));
+    for (DevBuf* b : {&sv.in, &sv.recs, &sv.sort, &sv.pack, &sv.pool, &sv.img}) b->release();
+    sv.stage = 0;
+    sv.n = sv.kept = sv.n_pool = sv.n_ovfl = sv.pages = 0;
+    sv.refused = nullptr;
+    return LGW_OK;
+}
+
+extern "C" int lgw_usage_save_last_ms(lgw_engine* e, float ms[6]) {
+    if (!e || !ms) return LGW_ERR_ARG;
+    for (int k = 0; k < 6; ++k) ms[k] = e->save.ms[k];
     return LGW_OK;
 }
 

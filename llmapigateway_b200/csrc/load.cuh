@@ -133,6 +133,13 @@ LGW_LOAD uint32_t local_size(uint32_t P, uint32_t U) {
     const uint32_t K = M + (P - M) % (U - 4);
     return K <= X ? K : M;
 }
+// the same for a cell of an index b-tree page: its own maximum local size X
+LGW_LOAD uint32_t index_local_size(uint32_t P, uint32_t U) {
+    const uint32_t X = ((U - 12) * 64 / 255) - 23, M = ((U - 12) * 32 / 255) - 23;
+    if (P <= X) return P;
+    const uint32_t K = M + (P - M) % (U - 4);
+    return K <= X ? K : M;
+}
 
 // Sequential reader of one cell's payload: the local part, then each overflow page's U - 4 bytes after its next-page number.
 struct PayCursor { const uint8_t* p; uint32_t left, next; bool bad; };

@@ -171,6 +171,198 @@ def read_tokens_usage_snapshot(db_path, alloc, free) -> dict:
     return {"buf": buf, "size": got, "page_size": ps, "n_pages": n_pages, "root": int(root), "seq": int(seq[0] or 0)}
 
 
+SAVE_TEXT_NULL, SAVE_TEXT_BAD = 0xFFFFFFFF, 0xFFFFFFFE     # lgw_save_text lengths (include/llmgw_b200.h)
+SQL_MAX_LENGTH = 1_000_000_000      # SQLite's default SQLITE_MAX_LENGTH: a longer text is not stored either
+
+
+class SaveText(C.Structure):
+    """lgw_save_text: text k of a table is bytes blob[off[k]:off[k] + len[k]], or NULL / not storable"""
+    _fields_ = [("blob", C.c_void_p), ("off", C.c_void_p), ("len", C.c_void_p), ("n", C.c_uint32), ("pad", C.c_uint32)]
+
+
+def _save_text_table(texts: list) -> tuple:
+    """(SaveText, the arrays it points into) for a list of str | None: UTF-8 bytes, NULL for None, BAD for a str that is not
+    encodable as UTF-8 (a lone surrogate) or longer than SQL_MAX_LENGTH bytes"""
+    raw, lens = [], np.empty(len(texts), np.uint32)
+    for k, s in enumerate(texts):
+        if s is None:
+            b, lens[k] = b"", SAVE_TEXT_NULL
+        else:
+            try:
+                b = s.encode("utf-8")
+            except UnicodeEncodeError:
+                b = None
+            if b is None or len(b) > SQL_MAX_LENGTH:
+                b, lens[k] = b"", SAVE_TEXT_BAD
+            else:
+                lens[k] = len(b)
+        raw.append(b)
+    off = np.zeros(len(texts) + 1, np.uint64)
+    np.cumsum([len(b) for b in raw], out=off[1:])
+    blob = np.frombuffer(b"".join(raw) or b"\0", np.uint8)
+    t = SaveText(blob.ctypes.data, off.ctypes.data, lens.ctypes.data, len(texts), 0)
+    return t, (blob, off, lens)
+
+
+def _varint(v: int) -> bytes:
+    if v >> 56:
+        out = [v & 0xFF]
+        v >>= 8
+        for i in range(8):
+            out.append((v & 0x7F) | 0x80)
+            v >>= 7
+        return bytes(reversed(out))
+    out = [v & 0x7F]
+    v >>= 7
+    while v:
+        out.append((v & 0x7F) | 0x80)
+        v >>= 7
+    return bytes(reversed(out))
+
+
+def _sql_record(values) -> bytes:
+    """a SQLite record of ints, strs and None (schema format 4)"""
+    types, body = [], b""
+    for v in values:
+        if v is None:
+            types.append(0)
+        elif isinstance(v, int):
+            if v in (0, 1):
+                types.append(8 + v)
+                continue
+            n, t = next((n, t) for n, t in ((1, 1), (2, 2), (3, 3), (4, 4), (6, 5), (8, 6)) if -(1 << (8 * n - 1)) <= v < 1 << (8 * n - 1))
+            types.append(t)
+            body += v.to_bytes(n, "big", signed=True)
+        else:
+            b = v.encode("utf-8")
+            types.append(13 + 2 * len(b))
+            body += b
+    head = b"".join(_varint(t) for t in types)
+    return _varint(len(head) + 1) + head + body        # (the schema's headers are short: their size takes one byte)
+
+
+def _leaf_page(rows, ps: int, first: bool) -> bytes:
+    """a table leaf page holding (rowid, record) cells that fit it without spilling; page 1 keeps its first 100 bytes for the
+    file header"""
+    hdr = 100 if first else 0
+    page = bytearray(ps)
+    at = ps
+    for k, (rowid, rec) in enumerate(rows):
+        cell = _varint(len(rec)) + _varint(rowid) + rec
+        at -= len(cell)
+        page[at:at + len(cell)] = cell
+        page[hdr + 8 + 2 * k:hdr + 10 + 2 * k] = at.to_bytes(2, "big")
+    assert hdr + 8 + 2 * len(rows) <= at
+    page[hdr] = 13
+    page[hdr + 3:hdr + 5] = len(rows).to_bytes(2, "big")
+    page[hdr + 5:hdr + 7] = (at & 0xFFFF).to_bytes(2, "big")
+    return bytes(page)
+
+
+def _sink_schema() -> list:
+    """(type, name, tbl_name, sql) of the sqlite_schema rows SqliteUsageSink creates, as the installed sqlite3 stores them"""
+    from .gateway import SqliteUsageSink
+    sink = SqliteUsageSink(":memory:")
+    try:
+        return sink.conn.execute("SELECT type, name, tbl_name, sql FROM sqlite_schema ORDER BY rowid").fetchall()
+    finally:
+        sink.conn.close()
+
+
+def _head_pages(ps: int, n_pages: int, table_root: int, index_root: int, seq: int) -> bytes:
+    """pages 1 (the 100-byte header and sqlite_schema) and 2 (sqlite_sequence) of a saved file"""
+    import sqlite3
+    roots = {"tokens_usage": table_root, "sqlite_sequence": 2, "idx_tokens_usage_timestamp": index_root}
+    schema = [(k + 1, _sql_record((ty, name, tbl, roots[name], sql))) for k, (ty, name, tbl, sql) in enumerate(_sink_schema())]
+    p1 = bytearray(_leaf_page(schema, ps, True))
+    v = sqlite3.sqlite_version_info
+    h = bytearray(100)
+    h[0:16] = b"SQLite format 3\x00"
+    h[16:18] = (ps if ps < 65536 else 1).to_bytes(2, "big")
+    h[18] = h[19] = 1                                      # rollback journal
+    h[21:24] = bytes((64, 32, 32))
+    h[24:28] = (1).to_bytes(4, "big")                      # file change counter
+    h[28:32] = n_pages.to_bytes(4, "big")
+    h[40:44] = (1).to_bytes(4, "big")                      # schema cookie
+    h[44:48] = (4).to_bytes(4, "big")                      # schema format
+    h[56:60] = (1).to_bytes(4, "big")                      # UTF-8
+    h[92:96] = (1).to_bytes(4, "big")                      # version-valid-for == the change counter
+    h[96:100] = (v[0] * 1000000 + v[1] * 1000 + v[2]).to_bytes(4, "big")
+    p1[:100] = h
+    p2 = _leaf_page([(1, _sql_record(("tokens_usage", seq)))] if seq > 0 else [], ps, False)
+    return bytes(p1) + p2
+
+
+def _check_page_size(page_size) -> None:
+    if isinstance(page_size, bool) or not isinstance(page_size, int) or not 1024 <= page_size <= 65536 or page_size & (page_size - 1):
+        raise ValueError(f"page_size {page_size!r}: a power of two in [1024, 65536]")
+
+
+class _ReplaceLock:
+    """Held while a save replaces the file at db_path: an EXCLUSIVE lock on the file there (SQLite rolls back a hot journal
+    when it takes it), nothing when there is none.  A WAL-mode file is refused before any connection is opened; a lock another
+    connection holds raises sqlite3.OperationalError at once."""
+
+    def __init__(self, db_path):
+        self.db_path, self.conn = db_path, None
+
+    def __enter__(self):
+        import os
+        import sqlite3
+        from urllib.parse import quote
+        if not os.path.exists(self.db_path):
+            return self
+        with open(self.db_path, "rb") as f:
+            head = f.read(100)
+        if len(head) >= 20 and head[:16] == b"SQLite format 3\x00" and 2 in (head[18], head[19]):
+            raise UsageDbNotModelled("the file at the path is in WAL mode: a save writes rollback-journal files only")
+        self.conn = sqlite3.connect(f"file:{quote(os.fspath(self.db_path))}?mode=rw", uri=True, isolation_level=None, timeout=0)
+        try:
+            self.conn.execute("BEGIN EXCLUSIVE")
+        except BaseException:
+            self.conn.close()
+            raise
+        return self
+
+    def __exit__(self, *exc):
+        if self.conn is not None:
+            self.conn.close()                     # (ends the transaction; the lock was on the file that has been replaced)
+
+
+def _write_replace(db_path, data) -> None:
+    """data to a temporary file next to db_path, fsync'd, moved over db_path with os.replace, then the directory fsync'd.  A
+    replaced file's permission bits carry over.  On a failure the temporary file is removed and db_path is as it was."""
+    import os
+    import tempfile
+    path = os.path.abspath(os.fspath(db_path))
+    d = os.path.dirname(path)
+    try:
+        mode = os.stat(path).st_mode & 0o7777
+    except FileNotFoundError:
+        umask = os.umask(0)
+        os.umask(umask)
+        mode = 0o666 & ~umask
+    fd, tmp = tempfile.mkstemp(prefix="." + os.path.basename(path) + ".", suffix=".saving", dir=d)
+    try:
+        with os.fdopen(fd, "wb") as f:
+            f.write(data)
+            f.flush()
+            os.fchmod(f.fileno(), mode)
+            os.fsync(f.fileno())
+        os.replace(tmp, path)
+    except BaseException:
+        try:
+            os.unlink(tmp)
+        except FileNotFoundError:
+            pass
+        raise
+    dfd = os.open(d, os.O_RDONLY)
+    try:
+        os.fsync(dfd)
+    finally:
+        os.close(dfd)
+
+
 def _utf8_or_none(b: bytes):
     try:
         return b.decode("utf-8")
@@ -212,6 +404,7 @@ class UsageTable:
     _dev_cap = 0
     _ts_range = None
     rejected_ids = np.zeros(0, np.int64)      # ids of the records the last load_tokens_usage_db refused
+    save_refused_ids = np.zeros(0, np.int64)  # ids of the records the last save_tokens_usage_db did not write
 
     def __init__(self, engine):
         self.eng = engine
@@ -391,6 +584,72 @@ class UsageTable:
         ms = (C.c_float * 4)()
         self.eng._ck(self._lib.lgw_usage_load_last_ms(self.eng._h, C.byref(ms)), "usage_load_last_ms")
         return {"copy": ms[0], "decode": ms[1], "dictionary": ms[2], "compaction": ms[3]}
+
+    # -- saving the table as a tokens_usage file ---------------------------------------------------------------------------
+    def save_tokens_usage_db(self, db_path, page_size: int = 4096) -> int:
+        """Write every record of the table (pending rows included: _upload() first) to a new `tokens_usage` SQLite file at
+        db_path, laid out on the device (csrc/save.cuh); the number written.  The file has SqliteUsageSink's schema, its
+        `tokens_usage` rows in id order with rowid = id (gaps kept), the timestamps as datetime.isoformat() text, costs as
+        8-byte REALs bit for bit (NaN as NULL), sqlite_sequence holding _seq (no row when it is 0) and a complete
+        idx_tokens_usage_timestamp; load_tokens_usage_db reads it back as this table.
+        A record the file cannot hold -- a model or provider that is not encodable as UTF-8, a timestamp with no isoformat text
+        (only load_columns can give one) -- is not written: its id goes to `save_refused_ids` and a warning is logged.
+        The file is written next to db_path, fsync'd and moved into place with os.replace.  An existing file is first locked
+        EXCLUSIVE through sqlite3 (which rolls back a hot journal) until it is replaced.  A busy lock (sqlite3.OperationalError),
+        a WAL-mode file there or a file of LOAD_MAX_BYTES or more (UsageDbNotModelled), a page_size that is not a power of two
+        in [1024, 65536] (ValueError) or any other failure leave the old file, and the table, as they were.  Replacing a file
+        that another connection still has open (a live SqliteUsageSink) is the caller's to avoid: that connection keeps
+        writing to the replaced file, and its rows are lost."""
+        _check_page_size(page_size)
+        self._upload()
+        n = int(self._host["ts_us"].size)
+        models, _m = _save_text_table(self._names)
+        codes: dict = {None: 0}
+        prov = np.fromiter((codes.setdefault(p, len(codes)) for p in self._providers), np.int32, count=n)
+        providers, _p = _save_text_table(list(codes))
+        ids = np.ascontiguousarray(self._ids[:n], np.int64)
+        with _ReplaceLock(db_path):
+            try:
+                out = np.zeros(5, np.uint64)
+                self._save_call("plan", self._save_cols(), n, ids.ctypes.data_as(C.c_void_p), prov.ctypes.data_as(C.c_void_p),
+                                C.byref(models), C.byref(providers), page_size, out.ctypes.data_as(C.c_void_p))
+                pages, table_root, index_root, kept, refused_n = (int(x) for x in out)
+                if pages * page_size >= LOAD_MAX_BYTES:
+                    raise UsageDbNotModelled(f"a file of {pages * page_size} bytes: load_tokens_usage_db reads files below 2^33 bytes")
+                buf = self._save_alloc(pages * page_size)
+                try:
+                    refused = np.zeros(refused_n, np.int64)
+                    self._save_call("write", buf.ctypes.data_as(C.c_void_p), refused.ctypes.data_as(C.c_void_p))
+                    buf[:2 * page_size] = np.frombuffer(_head_pages(page_size, pages, table_root, index_root, self._seq), np.uint8)
+                    _write_replace(db_path, memoryview(buf)[:pages * page_size])
+                finally:
+                    self._save_free(buf)
+            finally:
+                self._save_call("release")
+        self.save_refused_ids = refused
+        if refused.size:
+            logging.warning(f"save_tokens_usage_db: {refused.size} records the file cannot hold were not written "
+                            "(a text that is not UTF-8, or a timestamp with no isoformat text); their ids are in save_refused_ids")
+        return kept
+
+    # the save's seams: a CPU stand-in replaces these with the host build of csrc/save.cuh and numpy buffers
+    def _save_call(self, step: str, *args):
+        self.eng._ck(getattr(self._lib, "lgw_usage_save_" + step)(self.eng._h, *args), "usage_save_" + step)
+
+    def _save_cols(self):
+        return (C.c_void_p * 8)(*[self._dev_ptrs[c].value for c in self.COLS])
+
+    def _save_alloc(self, nbytes: int) -> np.ndarray:
+        return self.eng.alloc_pinned(nbytes)
+
+    def _save_free(self, buf: np.ndarray):
+        self._lib.lgw_free_pinned(self.eng._h, C.c_void_p(buf.ctypes.data))
+
+    def save_last_ms(self) -> dict:
+        """device times of the last save_tokens_usage_db, milliseconds"""
+        ms = (C.c_float * 6)()
+        self.eng._ck(self._lib.lgw_usage_save_last_ms(self.eng._h, C.byref(ms)), "usage_save_last_ms")
+        return dict(zip(("upload", "keep", "sort", "pack", "write", "download"), ms))
 
     def _grow(self, key: str, a: np.ndarray, new: np.ndarray) -> np.ndarray:
         """a followed by new, as an exact-length view of a buffer of this table with room to grow (doubling): when a is the
