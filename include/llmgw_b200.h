@@ -130,7 +130,9 @@ int lgw_engine_set_stream(lgw_engine* e, void* cuda_stream);
 /* ---- streams ------------------------------------------------------------------------------------
  * One slot = one upstream attempt of make_llm_request(..., is_streaming=True)
  * (llm_gateway_core/services/request_handler.py:8).  http_status is the upstream response status
- * (:25-30): >= 400 marks the attempt failed at once and the host keeps the body as error detail. */
+ * (:25-30): >= 400 marks the attempt failed at once and the host keeps the body as error detail.
+ * Stream-ordered on the engine stream: returns without waiting for the GPU; the arrays are copied
+ * before it returns, so the caller may reuse them at once. */
 int lgw_streams_open(lgw_engine* e, const uint32_t* slots, const int32_t* http_status, uint32_t n);
 int lgw_streams_state(lgw_engine* e, const uint32_t* slots, uint32_t n, lgw_stream_state* out);
 /* error detail of a failed attempt: the text the reference stores at request_handler.py:51,87

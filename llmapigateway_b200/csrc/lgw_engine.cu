@@ -104,6 +104,10 @@ struct lgw_engine {
     uint32_t* d_rowq_count = nullptr; RowEvent* d_rowq = nullptr;
     StepScratch scratch{};          // per-step scratch (sized by max_step_chunks / max_streams)
     uint32_t* d_slots = nullptr; int32_t* d_status = nullptr; StreamState* d_state_stage = nullptr;   // slot lists of open / state / close
+    struct Open {                   // lgw_streams_open is stream-ordered: the caller's lists are copied here first, so they are free on return
+        HostBuf h;                  // page-locked: slots[max_streams] ++ status[max_streams]
+        cudaEvent_t done = nullptr; bool pending = false;   // recorded after the uploads; waited for before the staging is written again
+    } open;
     DevBuf details;                 // staging of lgw_streams_details
     struct Step {
         uint8_t *d_in = nullptr, *d_out = nullptr;      // staging for the host-pointer entry point
@@ -270,7 +274,9 @@ extern "C" int lgw_engine_create(int device, const lgw_limits* limits, lgw_engin
     ALLOC(e->step.d_seg_out, S * sizeof(SegResult));
     ALLOC(e->d_slots, S * 4); ALLOC(e->d_status, S * 4); ALLOC(e->d_state_stage, S * sizeof(StreamState));
 #undef ALLOC
-    if ((r = scratch_alloc(e->scratch, S, B, [e](auto*& p, size_t bytes) { return dev_alloc(e, p, bytes); })) != cudaSuccess) return fail("scratch_alloc", r);
+    if ((r = e->open.h.reserve(S * 8)) != cudaSuccess) return fail("cudaHostAlloc", r);
+    if ((r = new_events(e, &e->open.done, 1, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", r);
+    if ((r = scratch_alloc(e->scratch, S, [e](auto*& p, size_t bytes) { return dev_alloc(e, p, bytes); })) != cudaSuccess) return fail("scratch_alloc", r);
     if ((r = cudaMemset(e->t.state, 0, S * sizeof(StreamState))) != cudaSuccess) return fail("cudaMemset", r);
     if ((r = cudaMemset(e->d_rowq_count, 0, 16)) != cudaSuccess) return fail("cudaMemset", r);
     const char* m = getenv("LGW_FORCE_GENERAL");
@@ -304,16 +310,27 @@ extern "C" int lgw_engine_set_mode(lgw_engine* e, int mode) {     // 0 fast+fix-
     return LGW_OK;
 }
 
+// Stream-ordered: returns once the work is enqueued, without waiting for the GPU (a serving loop enqueues the next step behind
+// it while earlier work still runs).  The caller's arrays are copied into the engine's page-locked staging first, so the caller
+// may reuse or free them on return, pinned or not; the staging itself is written again only after its last upload is done.
 extern "C" int lgw_streams_open(lgw_engine* e, const uint32_t* slots, const int32_t* http_status, uint32_t n) {
     if (!e || !slots || !http_status) return LGW_ERR_ARG;
     if (n == 0) return LGW_OK;
-    TRY(stage_slots(e, slots, n));
-    CK(e, cudaMemcpyAsync(e->d_status, http_status, n * 4, cudaMemcpyHostToDevice, e->stream));
+    if (n > e->lim.max_streams) { e->err = "more slots than max_streams"; return LGW_ERR_CAPACITY; }
+    TRY(check_slots(e, slots, n));
+    CK(e, cudaSetDevice(e->device));
+    if (e->open.pending) { CK(e, cudaEventSynchronize(e->open.done)); e->open.pending = false; }
+    uint32_t* h_slots = e->open.h.as<uint32_t>();
+    int32_t* h_status = reinterpret_cast<int32_t*>(h_slots + e->lim.max_streams);
+    memcpy(h_slots, slots, (size_t)n * 4); memcpy(h_status, http_status, (size_t)n * 4);
+    CK(e, cudaMemcpyAsync(e->d_slots, h_slots, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(e, cudaMemcpyAsync(e->d_status, h_status, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(e, cudaEventRecord(e->open.done, e->stream));
+    e->open.pending = true;
     k_streams_open<<<(n + 127) / 128, 128, 0, e->stream>>>(e->t, e->d_slots, e->d_status, n);
     ++e->launches;
     if (e->text.on) { k_text_open<<<(n + 127) / 128, 128, 0, e->stream>>>(e->text.tap, e->d_slots, n); ++e->launches; }
     CK(e, cudaGetLastError());
-    CK(e, cudaStreamSynchronize(e->stream));
     return LGW_OK;
 }
 

@@ -1,4 +1,4 @@
-// Bulk path of the SSE step, round 2:  k_prime2 -> k_relay2 -> k_commit2.
+// Bulk path of the SSE step, round 2:  k_relay2 -> k_commit2.
 // (included from sse_kernels.cuh, inside namespace lgw)
 //
 // What changed against round 1 (relay_kernels.cuh, thread-per-chunk walk of a staged tile):
@@ -64,7 +64,7 @@
 #define R2_TILE 3072u                   /* a multiple of 512 (the fast loop walks whole 512-byte windows of a tile) */
 #endif
 #ifndef R2_NBUF
-#define R2_NBUF 2u                      /* ring depth per warp.  2 x 3 KiB x 16 warps = 96 KiB: with the 28 KiB of tables the block takes the 132 KiB
+#define R2_NBUF 2u                      /* ring depth per warp.  2 x 3 KiB x 16 warps = 96 KiB: with the 33 KiB of tables the block takes the 132 KiB
                                            carve-out and leaves ~96 KiB of L1 for the out-of-line paths' local memory (672 B of stack per thread);
                                            on the H100 a 3-deep ring (144 KiB) was no faster (DESIGN 9.8) */
 #endif
@@ -93,7 +93,7 @@ struct Tpl2 {
 // state: 0 empty, 1 being written, 2 ready.
 struct TemplateCache2 {
     uint32_t state[R2_SLOTS];
-    uint32_t hits[R2_SLOTS];         // events matched per slot (decayed in k_prime2)
+    uint32_t hits[R2_SLOTS];         // events matched per slot (decayed once per launch set: tpl_cache_upkeep)
     uint32_t general;                // events that matched no slot
     uint32_t lock;                   // publication lock
     uint32_t _pad[2];
@@ -114,6 +114,7 @@ struct R2Shared {
     uint32_t general;
     uint32_t dflt, fast_ready;
     uint32_t learn_lock;                             // one warp of the block learns a template at a time
+    uint32_t plan_win[R2_WARPS][3][32];              // per warp: relay_begin / seg_end / kept_end of 32 consecutive segments (SegStatic)
     StepArgs args;                                   // the kernel's arguments (read through a pointer by the out-of-line paths: taking the
                                                      //   address of the parameter itself would move it to local memory)
     alignas(4) uint8_t cls[256];
@@ -459,6 +460,89 @@ R2_DEV_NOINLINE void decode_string_span(const RD& rd, uint32_t p, uint32_t n, ch
     dlen = (uint8_t)len; dflags = (uint8_t)flags;
 }
 
+// ---- the static plan of a segment ----------------------------------------------------------------------------------------
+// Where a segment's bulk region lies, and whether its stream is SPECULATED to commit on its first non-empty chunk (a fresh
+// stream; the bulk kernel verifies, k_commit2 applies or falls back).  A pure function of the segment's chunks, their offsets
+// and the stream's state at the start of the launch set: k_relay2's warps and the segment's k_commit2 warp each compute it,
+// and they must reach the same verdict, so this is the one place that decides it.
+struct SegStatic {
+    uint32_t resume_chunk;     // first chunk the sequential path would have to (re)do
+    uint32_t relay_begin;      // byte offset where the bulk region starts (tap view); seg_end when none
+    uint32_t seg_end;          // byte offset of the end of the segment
+    uint32_t emit_chunk_begin;
+    uint32_t kept_chunk;       // the speculated stream's first non-empty chunk (request_handler.py:69-95); R2_NONE: no speculation
+    uint32_t kept_end;         // byte offset of the end of the kept chunk = where the handler's text starts; 0: none
+    uint32_t irregular;        // 1: no bulk region, k_commit2 redoes [resume_chunk, end)
+};
+R2_DEV SegStatic seg_static(const uint32_t* chunk_off, uint32_t c0, uint32_t c1, uint32_t phase, uint32_t flags, uint32_t carry_a_len) {
+    SegStatic p;
+    p.seg_end = __ldg(chunk_off + c1); p.relay_begin = p.seg_end; p.irregular = 0;
+    p.kept_chunk = R2_NONE; p.kept_end = 0;
+    p.resume_chunk = c0; p.emit_chunk_begin = phase == PH_COMMITTED ? c0 : c1;
+    if (phase == PH_COMMITTED && c0 < c1) {
+        if ((flags & SF_SYNCED) && carry_a_len == 0) p.relay_begin = __ldg(chunk_off + c0);
+        else p.irregular = 1;
+    } else if (phase == PH_PRIMING && c0 < c1) {
+        uint32_t c = c0;
+        while (c < c1 && __ldg(chunk_off + c + 1) == __ldg(chunk_off + c)) ++c;     // empty chunks are never yielded (:60-63)
+        if (c < c1 && carry_a_len == 0) {
+            p.kept_chunk = c; p.kept_end = __ldg(chunk_off + c + 1); p.relay_begin = __ldg(chunk_off + c); p.emit_chunk_begin = c;
+        } else if (c < c1) p.irregular = 1;                                    // an event is open from an earlier step
+    }
+    return p;
+}
+// segment `seg`'s static plan into the warp's window, column i
+R2_DEV void put_plan(const StepArgs& a, uint32_t* win, uint32_t i, uint32_t seg) {
+    const uint32_t c0 = __ldg(a.seg_chunk + seg), c1 = __ldg(a.seg_chunk + seg + 1);
+    const StreamHdr* h = &a.t.state[__ldg(a.seg_slot + seg)].h;
+    const SegStatic p = seg_static(a.chunk_off, c0, c1, h->phase, h->flags, h->carry_a_len);
+    win[i] = p.relay_begin; win[32 + i] = p.seg_end; win[64 + i] = p.kept_end;
+}
+// the window holds segments [lo, lo + 32): lane i computes segment lo + i
+R2_DEV_NOINLINE void load_plans(const StepArgs* ap, uint32_t* win, uint32_t lane, uint32_t lo) {
+    __syncwarp();                                                              // (every lane is done with the old window)
+    if (lo + lane < ap->n_segs) put_plan(*ap, win, lane, lo + lane);
+    __syncwarp();
+}
+// The first segment whose text ends past byte x (the one that holds x; n_segs: none), with the warp's plan window filled from
+// at most 31 segments before it.  Streams of a step tend to be of similar length, so the first round reads the 32 segments
+// around the one the byte position suggests, each lane its candidate's whole plan: when they bracket the answer, that round
+// was the search and the window load at once.  Otherwise strided rounds (two dependent reads each) narrow the answer down,
+// and the window is loaded from it.
+// Returns (the segment, the window's first segment).
+R2_DEV_NOINLINE uint2 first_segment(const StepArgs* ap, uint32_t* win, uint32_t lane, uint32_t x) {
+    const StepArgs& a = *ap;
+    const uint32_t n = a.n_segs;
+    const uint32_t nb = a.n_bytes - a.tile_base;
+    const uint32_t g = nb ? (uint32_t)((unsigned long long)n * (x - a.tile_base) / nb) : 0u;
+    const uint32_t w0 = n <= 32u ? 0u : r2_min(g > 16u ? g - 16u : 0u, n - 32u);
+    if (w0 + lane < n) put_plan(a, win, lane, w0 + lane);
+    __syncwarp();
+    const bool past = w0 + lane < n && win[32 + lane] > x;
+    const uint32_t pm = __ballot_sync(R2_FULL, past);
+    uint32_t lo, hi;
+    if (pm) {
+        const uint32_t k = (uint32_t)__ffs(pm) - 1u;
+        if (k || w0 == 0u) return make_uint2(w0 + k, w0);                                    // bracketed (or the very first segment)
+        lo = 0; hi = w0;
+    } else {
+        if (w0 + 32u >= n) return make_uint2(n, w0);                                       // every segment ends at or before x
+        lo = w0 + 32u; hi = n;
+    }
+    while (lo < hi) {
+        const uint32_t s = lo + (uint32_t)((unsigned long long)(hi - lo) * lane / 32u);     // (nondecreasing in the lane)
+        const bool e_past = __ldg(a.chunk_off + __ldg(a.seg_chunk + s + 1)) > x;
+        const uint32_t m = __ballot_sync(R2_FULL, e_past);
+        if (!m) { lo = __shfl_sync(R2_FULL, s, 31) + 1u; continue; }
+        const uint32_t k = (uint32_t)__ffs(m) - 1u;
+        const uint32_t sk = __shfl_sync(R2_FULL, s, (int)k), sp = __shfl_sync(R2_FULL, s, k ? (int)k - 1 : 0);
+        hi = sk;
+        if (k) lo = sp + 1u;
+    }
+    load_plans(ap, win, lane, lo);
+    return make_uint2(lo, lo);
+}
+
 // ---- helpers of the walk ---------------------------------------------------------------------------------------------------
 R2_DEV void flush_counts(R2Ctx& c) {
     if (c.lane == 0 && c.seg != R2_NONE) {
@@ -616,18 +700,17 @@ R2_DEV_NOINLINE void learn_template(const StepArgs* ap, R2Shared* sh, R2Io io, U
     __syncwarp();
 }
 
-// Enter segment `seg`; `from` = the warp's range start when the segment's bytes begin before it, else the segment's first
-// byte.  Sets the text range and the first event start this warp owns in it; false: the warp owns nothing here.
-R2_DEV bool enter_segment(R2Ctx& c, uint32_t seg, uint32_t from, uint32_t range_hi) {
+// Enter segment `seg` (static plan: bulk region [tb, te), kept = end of the kept chunk, 0: none); `from` = the warp's range
+// start when the segment's bytes begin before it, else the segment's first byte.  Sets the text range and the first event start
+// this warp owns in it; false: the warp owns nothing here.
+R2_DEV bool enter_segment(R2Ctx& c, uint32_t seg, uint32_t tb, uint32_t te, uint32_t kept, uint32_t from, uint32_t range_hi) {
     const SegPlan* pl = c.a->s.plan + seg;
     c.seg = seg; c.ev_a = c.ev_b = c.a_usage = 0; c.high = 0; c.in_kept = 0; c.primed = 0; c.kept_tried = 0;
-    const uint32_t tb = pl->relay_begin, te = pl->seg_end;
     c.tb = tb; c.te = te;
-    const uint32_t kept = pl->kept_chunk != 0xFFFFFFFFu ? pl->kept_end : 0u;
     c.kept_end = kept;
     c.pos = te; c.walk_lo = te;
     c.t = 0;
-    // `irregular` is the one plan field other warps write while this kernel runs (mark_irregular): one lane reads it and hands
+    // `irregular` is a finding other warps write while this kernel runs (mark_irregular): one lane reads it and hands
     // it to all -- lanes reading it on their own could see different values and part ways before the next collective
     uint32_t irr = 0;
     if (c.lane == 0) irr = *(volatile const uint32_t*)&pl->irregular;
@@ -1044,7 +1127,7 @@ R2_DEV bool walk_segment(R2Ctx& c, const uint32_t range_hi) {
                 c.in_kept = 0;
                 continue;
             }
-            if (lane == 0) c.a->s.plan[c.seg].tail_start = c.s_open;           // the open event is the new carry
+            if (lane == 0) c.a->s.plan[c.seg].tail_start = c.s_open + 1u;      // the open event is the new carry
             return false;
         }
         if (c.s_open >= range_hi && c.pos == c.s_open && !c.in_kept) return true;   // the open event starts in the next warp's range
@@ -1139,8 +1222,10 @@ k_relay2(StepArgs a, uint32_t n_tiles_total, uint32_t tiles_per_warp, uint32_t b
     TemplateCache2* tc = a.s.tpl_cache2;
     UsageRaw* block_raw = sh->raw_tpl;
 
-    // ---- block prologue: recogniser tables, barriers, the first tiles (all independent of k_prime2, which may still run) ----
+    // ---- block prologue: recogniser tables, barriers, the first tiles.  This is the launch set's first kernel, ordered behind the
+    // previous one's k_commit2 (and any k_streams_open) by the stream: nothing to wait for ----
     griddep_launch();
+    if (R2_BID == 0 && tid == 0 && a.reset_rows) *a.rowq_count = 0;        // (only k_commit2 appends rows, after this kernel)
     for (uint32_t k = tid; k < 64 + LGW_LEAN_ROWS * 8; k += R2_THREADS) {
         if (k < 64) reinterpret_cast<uint32_t*>(sh->cls)[k] = reinterpret_cast<const uint32_t*>(lean_tables().cls)[k];
         else reinterpret_cast<uint32_t*>(sh->trans)[k - 64] = reinterpret_cast<const uint32_t*>(lean_tables().trans)[k - 64];
@@ -1159,8 +1244,6 @@ k_relay2(StepArgs a, uint32_t n_tiles_total, uint32_t tiles_per_warp, uint32_t b
     c.base = base0 + t_first * R2_TILE;
     c.n_tiles = t_first >= n_tiles_total ? 0u : r2_min(tiles_per_warp, n_tiles_total - t_first);
     pipe_start(c);
-    // ---- from here on: what k_prime2 wrote (plans, tile table, template cache upkeep) ----
-    griddep_wait();
     if (tid < R2_SLOTS) { sh->slot_state[tid] = (*(volatile uint32_t*)&tc->state[tid] == 2u) ? 2u : 0u; sh->slot_gidx[tid] = tid; }
     __syncthreads();
     for (uint32_t s = 0; s < R2_SLOTS; ++s) {
@@ -1193,14 +1276,21 @@ k_relay2(StepArgs a, uint32_t n_tiles_total, uint32_t tiles_per_warp, uint32_t b
     if (c.n_tiles == 0) return;
     const uint32_t range_lo = r2_max(c.base, a.tile_base);          // (tile_base = first byte of this launch; a slice starts inside tile 0)
     const uint32_t range_hi = r2_min(c.base + c.n_tiles * R2_TILE, a.n_bytes);
+    uint32_t* win = &sh->plan_win[warp][0][0];
+    const uint2 fs = first_segment(&sh->args, win, lane, range_lo);              // the segment that holds the range's first byte
+    const uint32_t seg0 = fs.x;
+    uint32_t win_lo = fs.y;
     pipe_advance(c);
 
-    for (uint32_t seg = a.s.tile_seg[t_first]; seg < a.n_segs; ++seg) {            // (the segment that holds the range's first byte: k_prime2's table)
-        const uint32_t seg_first = seg ? a.s.plan[seg - 1].seg_end : a.tile_base;
+    uint32_t seg_first = range_lo;                                                // (seg0's text begins at or before range_lo)
+    for (uint32_t seg = seg0; seg < a.n_segs; ++seg) {
         if (seg_first >= range_hi) break;
-        const bool done = enter_segment(c, seg, r2_max(range_lo, seg_first), range_hi) && walk_segment(c, range_hi);
+        if (seg - win_lo >= 32u) { win_lo = seg; load_plans(&sh->args, win, lane, seg); }   // the walk has left the window
+        const uint32_t i = seg - win_lo, tb = win[i], te = win[32 + i], kept = win[64 + i];
+        const bool done = enter_segment(c, seg, tb, te, kept, r2_max(range_lo, seg_first), range_hi) && walk_segment(c, range_hi);
         leave_segment(c, range_hi);
         if (done) break;
+        seg_first = te;
     }
     // ---- the rest of the range is copy only ----
     while (c.k + 1 < c.n_tiles) pipe_advance(c);
@@ -1211,54 +1301,21 @@ k_relay2(StepArgs a, uint32_t n_tiles_total, uint32_t tiles_per_warp, uint32_t b
     }
 }
 
-// ---- k_prime2 ------------------------------------------------------------------------------------------------------------------
-// thread i: the plan of segment i the bulk kernel works to.  Fresh streams are SPECULATED to commit on their first
-// non-empty chunk; the bulk kernel verifies, k_commit2 applies or falls back.  Thread 0 also looks after the template cache.
-R2_GLOBAL void k_prime2(StepArgs a) {
-    griddep_launch();
-    const uint32_t i = R2_BID * R2_NTHR + R2_TID;
-    if (i == 0) {
-        if (a.reset_rows) *a.rowq_count = 0;                                   // (the kernels after this one append rows)
-        TemplateCache2* tc = a.s.tpl_cache2;
-        uint32_t total = 0, full = 1, lo = 0;
-        for (uint32_t s = 0; s < R2_SLOTS; ++s) { total += tc->hits[s]; if (tc->state[s] != 2u) full = 0; if (tc->hits[s] < tc->hits[lo]) lo = s; }
-        // most events of the last steps matched no template although every slot is taken: forget the least useful one
-        // -- or one slot has not matched anything for many steps while events go unmatched
-        if (full && tc->general && (tc->hits[lo] == 0 || (tc->general > 64u && tc->general > total / 2u))) { tc->state[lo] = 0; tc->hits[lo] = 0; }
-        for (uint32_t s = 0; s < R2_SLOTS; ++s) tc->hits[s] >>= 1;
-        tc->general >>= 1;
-    }
-    if (i >= a.n_segs) return;
-    const uint32_t seg = i, c0 = a.seg_chunk[seg], c1 = a.seg_chunk[seg + 1];
-    const uint32_t slot = a.seg_slot[seg];
-    const StreamHdr st = a.t.state[slot].h;
-    SegPlan p;
-    p.seg_end = a.chunk_off[c1]; p.relay_begin = p.seg_end; p.irregular = 0; p.last_usage = 0; p.a_usage = 0;
-    p.n_events_a = p.n_events_b = p.n_usage_b = 0; p.tail_start = 0xFFFFFFFFu; p.cand_ps = 0;
-    p.kept_chunk = 0xFFFFFFFFu; p.kept_end = 0; p.prime_ok = 0;
-    p.resume_chunk = c0; p.emit_chunk_begin = (st.phase == PH_COMMITTED) ? c0 : c1;
-    if (st.phase == PH_COMMITTED && c0 < c1) {
-        if ((st.flags & SF_SYNCED) && st.carry_a_len == 0) p.relay_begin = a.chunk_off[c0];
-        else p.irregular = 1;
-    } else if (st.phase == PH_PRIMING && c0 < c1) {
-        uint32_t c = c0;
-        while (c < c1 && a.chunk_off[c + 1] == a.chunk_off[c]) ++c;          // empty chunks are never yielded (:60-63)
-        if (c < c1 && st.carry_a_len == 0) {
-            p.kept_chunk = c; p.kept_end = a.chunk_off[c + 1]; p.relay_begin = a.chunk_off[c]; p.emit_chunk_begin = c;
-        } else if (c < c1) p.irregular = 1;                                    // an event is open from an earlier step
-    }
-    a.s.plan[seg] = p;
-    // the byte tiles whose first byte lies in this segment: where the bulk kernel's warps start looking.  Tile 0 starts at
-    // tile_base & ~15, before the launch's first byte when a slice starts unaligned: the first segment WITH bytes claims it
-    // (b0 == tile_base), even when segments without bytes come before it -- else nobody writes tile_seg[0] and warp 0 starts
-    // from whatever an earlier launch left there, which may skip the text it owns
-    const uint32_t base0 = a.tile_base & ~15u;
-    const uint32_t b0 = a.chunk_off[c0], b1 = p.seg_end;
-    if (b1 > b0) {
-        uint32_t t_lo = b0 == a.tile_base ? 0u : (b0 - base0 + R2_TILE - 1) / R2_TILE;
-        const uint32_t t_hi = (b1 - 1 - base0) / R2_TILE;
-        for (uint32_t t = t_lo; t <= t_hi; ++t) a.s.tile_seg[t] = seg;
-    }
+#if R2_HOST_EMU
+// The emulator's step driver (tests/support/host_relay2.cpp) still launches a planning kernel before the bulk kernel, as the
+// device step did before each kernel began to compute its segments' static plans itself (seg_static): nothing is left for it.
+R2_GLOBAL void k_prime2(StepArgs) {}
+#endif
+
+// ---- template-cache upkeep: once per launch set, between its k_relay2 and the next launch set's (k_commit2's block 0) ----------------
+R2_DEV void tpl_cache_upkeep(TemplateCache2* tc) {
+    uint32_t total = 0, full = 1, lo = 0;
+    for (uint32_t s = 0; s < R2_SLOTS; ++s) { total += tc->hits[s]; if (tc->state[s] != 2u) full = 0; if (tc->hits[s] < tc->hits[lo]) lo = s; }
+    // most events of the last steps matched no template although every slot is taken: forget the least useful one
+    // -- or one slot has not matched anything for many steps while events go unmatched
+    if (full && tc->general && (tc->hits[lo] == 0 || (tc->general > 64u && tc->general > total / 2u))) { tc->state[lo] = 0; tc->hits[lo] = 0; }
+    for (uint32_t s = 0; s < R2_SLOTS; ++s) tc->hits[s] >>= 1;
+    tc->general >>= 1;
 }
 
 // ---- k_commit2 (one warp per segment) ----------------------------------------------------------------------------------------------
@@ -1374,9 +1431,14 @@ R2_DEV void commit_one(const StepArgs& a, uint32_t seg, uint32_t lane, uint8_t* 
         }
     }
     const bool any_empty = __any_sync(R2_FULL, empty);
+    // the plan the bulk kernel worked to (its chunk offsets were just read by the scan)
+    const SegStatic p = seg_static(a.chunk_off, c0, c1, st.phase, st.flags, st.carry_a_len);
     griddep_wait();                                       // (the bulk kernel's findings from here on)
-    const SegPlan p = a.s.plan[seg];                      // (resume_chunk is the segment's first chunk: k_prime2)
-    const uint2 fw = lane < 9u ? a.s.usage_fields[(size_t)seg * 9u + lane] : make_uint2(0u, 0xFFFFFFFFu);   // (requested with the plan, used when has_cand)
+    SegPlan* const fp = a.s.plan + seg;
+    const SegPlan f = *fp;
+    const uint2 fw = lane < 9u ? a.s.usage_fields[(size_t)seg * 9u + lane] : make_uint2(0u, 0xFFFFFFFFu);   // (requested with the findings, used when has_cand)
+    __syncwarp();
+    if (lane < sizeof(SegPlan) / 4) reinterpret_cast<uint32_t*>(fp)[lane] = 0u;   // read: zero again for the next launch set
     const StepIO io = make_io(a, slot, &st);
     uint32_t emit_begin = p.emit_chunk_begin;
     const bool speculated = p.kept_chunk != 0xFFFFFFFFu;
@@ -1384,9 +1446,9 @@ R2_DEV void commit_one(const StepArgs& a, uint32_t seg, uint32_t lane, uint8_t* 
         const uint8_t* __restrict__ d = a.data;
         // the winning usage event: its text (and, when the bulk kernel matched it against a usage template, where its fields sit)
         // is requested now, together with the chunk offsets below -- one round trip for all of it
-        const uint32_t ups = (uint32_t)(p.last_usage >> 32) - 1u, ulen = (uint32_t)p.last_usage;
-        const bool staged = p.last_usage && ulen <= LGW_PENDING_CAP && (uint64_t)ups + ulen <= a.n_bytes;
-        const bool has_cand = staged && p.cand_ps == ups + 1u;
+        const uint32_t ups = (uint32_t)(f.last_usage >> 32) - 1u, ulen = (uint32_t)f.last_usage;
+        const bool staged = f.last_usage && ulen <= LGW_PENDING_CAP && (uint64_t)ups + ulen <= a.n_bytes;
+        const bool has_cand = staged && f.cand_ps == ups + 1u;
         const uint2 fld = has_cand && lane < 8u ? fw : make_uint2(0u, 0xFFFFFFFFu);
         const uint32_t g_slot = __shfl_sync(R2_FULL, fw.x, 8), g_flags = __shfl_sync(R2_FULL, fw.y, 8);
         if (has_cand) {                                   // the template event's own UsageRaw, requested together with the text
@@ -1406,10 +1468,10 @@ R2_DEV void commit_one(const StepArgs& a, uint32_t seg, uint32_t lane, uint8_t* 
                 else for (uint32_t j = 0; j < 16u && o + j < a.n_bytes; ++j) stage[(k << 4) + j] = __ldg(d + o + j);
             }
         }
-        bool sequential = p.irregular || p.n_usage_b > 1 || any_empty;   // several usage candidates: let the exact path count them
-        if (st.phase == PH_PRIMING && !(speculated && p.prime_ok)) sequential = true;
-        if (!sequential && p.last_usage && !staged) sequential = true;
-        if (!sequential && p.tail_start == 0xFFFFFFFFu) sequential = true;                        // (nobody reached the end of the text)
+        bool sequential = p.irregular || f.irregular || f.n_usage_b > 1 || any_empty;   // several usage candidates: let the exact path count them
+        if (st.phase == PH_PRIMING && !(speculated && f.prime_ok)) sequential = true;
+        if (!sequential && f.last_usage && !staged) sequential = true;
+        if (!sequential && f.tail_start == 0u) sequential = true;                                // (nobody reached the end of the text)
         if (lane == 0) atomicAdd(&counts[sequential ? 0 : 1], 1u);
         if (sequential) {
             if (lane == 0) emit_begin = commit_sequential(io, a.data, a.chunk_off, p.resume_chunk, c1, (st.phase == PH_COMMITTED) ? p.resume_chunk : c1);
@@ -1424,9 +1486,9 @@ R2_DEV void commit_one(const StepArgs& a, uint32_t seg, uint32_t lane, uint8_t* 
             }
             const uint32_t nch = c1 - first, nby = p.seg_end - p.relay_begin;
             st.n_chunks_in += nch; st.n_chunks_emitted += nch; st.bytes_in += nby; st.bytes_emitted += nby;
-            st.n_events_a += p.n_events_a; st.n_events_b += p.n_events_b;
-            if (p.a_usage) st.flags |= SF_A_USAGE_BOUND;
-            if (p.last_usage) {                     // the last usage-bearing event wins (chat_logging.py:134-135)
+            st.n_events_a += f.n_events_a; st.n_events_b += f.n_events_b;
+            if (f.a_usage) st.flags |= SF_A_USAGE_BOUND;
+            if (f.last_usage) {                     // the last usage-bearing event wins (chat_logging.py:134-135)
                 if (lane == 0 && (st.flags & SF_PENDING)) commit_settle_pending(io);   // (a stash left by an older engine version of this stream)
                 __syncwarp();
                 if (has_cand) {
@@ -1441,7 +1503,7 @@ R2_DEV void commit_one(const StepArgs& a, uint32_t seg, uint32_t lane, uint8_t* 
                 }
             }
             // new carry = text after the last separator (both loops: SF_SYNCED)
-            const uint32_t tail = p.tail_start, n = p.seg_end - tail;
+            const uint32_t tail = f.tail_start - 1u, n = p.seg_end - tail;
             if (n > a.t.carry_cap) { st.carry_a_len = 0; st.flags |= SF_CARRY_OVERFLOW; }
             else { for (uint32_t k = lane; k < n; k += 32) io.carry_a[k] = d[tail + k]; st.carry_a_len = n; }
         }
@@ -1475,34 +1537,33 @@ k_commit2(StepArgs a) {
     if (seg < a.n_segs) commit_one(a, seg, lane, stage[warp], &stage_raw[warp], counts);
     __syncthreads();
     if (R2_TID < 4 && counts[R2_TID]) atomicAdd(a.s.counters + R2_TID, counts[R2_TID]);
+    if (R2_BID == 0 && R2_TID == 0) tpl_cache_upkeep(a.s.tpl_cache2);   // (segment 0's lane 0: past griddep_wait, the bulk kernel is done)
 }
 
 #if !R2_HOST_EMU
-// The three kernels of a step.  per_kernel = true: CUDA events between them (ev[1..3]) for the per-kernel times; false: the
-// bulk kernel and the commit kernel are launched with programmatic stream serialisation, so that each one's prologue (and
-// its launch latency) overlaps the kernel before it -- they wait (griddepcontrol.wait) before reading what that kernel wrote.
+// The two kernels of a launch set.  k_relay2 is launched plainly: stream order puts it behind the previous launch set and any
+// k_streams_open, whose writes (stream states, findings zeroed, template cache) it reads from its first instruction on.
+// per_kernel = true: CUDA events between the kernels (ev[1] = ev[0]: nothing runs before the bulk kernel); false: k_commit2 is
+// launched with programmatic stream serialisation, so that its prologue (and its launch latency) overlaps the bulk kernel -- it
+// waits (griddepcontrol.wait) before it reads what that kernel wrote.
 static inline cudaError_t launch_step_fast(const StepArgs& a, int sm_count, cudaStream_t stream, cudaEvent_t* ev, int* launched, bool per_kernel) {
     cudaError_t r;
     const uint32_t base0 = a.tile_base & ~15u;
     const uint32_t n_tiles = a.n_bytes > base0 ? (a.n_bytes - base0 + R2_TILE - 1) / R2_TILE : 0u;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    if (a.n_segs) { k_prime2<<<(a.n_segs + 127) / 128, 128, 0, stream>>>(a); ++*launched; }
     if (per_kernel && (r = cudaEventRecord(ev[1], stream)) != cudaSuccess) return r;
     if (n_tiles) {
         const uint32_t max_warps = (uint32_t)sm_count * R2_WARPS;
         const uint32_t tpw = (n_tiles + max_warps - 1) / max_warps;
         const uint32_t warps = (n_tiles + tpw - 1) / tpw;
         const uint32_t blocks = (warps + R2_WARPS - 1) / R2_WARPS;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(blocks); cfg.blockDim = dim3(R2_THREADS); cfg.dynamicSmemBytes = R2_SMEM_BYTES; cfg.stream = stream;
-        cfg.attrs = attr; cfg.numAttrs = per_kernel ? 0 : 1;
-        if ((r = cudaLaunchKernelEx(&cfg, k_relay2, a, n_tiles, tpw, base0)) != cudaSuccess) return r;
+        k_relay2<<<blocks, R2_THREADS, R2_SMEM_BYTES, stream>>>(a, n_tiles, tpw, base0);
         ++*launched;
-    }
+    } else if (a.reset_rows && (r = cudaMemsetAsync(a.rowq_count, 0, 4, stream)) != cudaSuccess) return r;   // (no bulk kernel to do it)
     if (per_kernel && (r = cudaEventRecord(ev[2], stream)) != cudaSuccess) return r;
     if (a.n_segs) {
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[0].val.programmaticStreamSerializationAllowed = 1;
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3((a.n_segs + R2_CWARPS - 1) / R2_CWARPS); cfg.blockDim = dim3(R2_CWARPS * 32); cfg.dynamicSmemBytes = 0; cfg.stream = stream;
         cfg.attrs = attr; cfg.numAttrs = per_kernel ? 0 : 1;
@@ -1514,4 +1575,3 @@ static inline cudaError_t launch_step_fast(const StepArgs& a, int sm_count, cuda
     return cudaGetLastError();
 }
 #endif
-

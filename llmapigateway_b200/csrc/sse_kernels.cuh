@@ -1,14 +1,16 @@
 // Kernels of the SSE step (sm_90a).  See DESIGN.md for the data layout and the roofline of each.
 //
-//   k_prime2   one thread per segment: the plan the bulk kernel works to; a fresh stream is speculated to commit
-//              on its first non-empty chunk.
-//   k_relay2   bulk kernel (relay2.cuh): one persistent block per SM, every warp owns a byte range; the re-emit is a
+// A launch set of the bulk path is two kernels, k_relay2 then k_commit2.  Neither needs a planning pass before it: each
+// segment's static plan (seg_static: its bulk region, and whether a fresh stream is speculated to commit on its first
+// non-empty chunk) is computed where it is used, and the bulk kernel's findings start at zero.
+//   k_relay2   bulk kernel (relay2.cuh): one persistent block per SM, every warp owns a byte range and finds its first segment
+//              itself (a 32-lane search over the segment table); the re-emit is a
 //              TMA pipeline through shared memory (cp.async.bulk in, cp.async.bulk out), the parse compares the
 //              staged bytes against periodic event templates, 16 bytes per lane, and reads the usage fields of
 //              template-following usage events straight from the matched value spans.
-//   k_commit2  one warp per segment: folds the bulk kernel's findings into the persistent stream state; streams
-//              the bulk kernel flagged irregular (or whose speculation failed) are redone sequentially with the
-//              exact machine.
+//   k_commit2  one warp per segment: folds the bulk kernel's findings into the persistent stream state and zeroes them;
+//              streams the bulk kernel flagged irregular (or whose speculation failed) are redone sequentially with the
+//              exact machine.  Its block 0 decays the template cache's hit counts for the next launch set.
 //   k_general  (mode 1 / fix-up) the exact sequential machine over whole segments.
 #pragma once
 #include <cuda_runtime.h>
@@ -70,21 +72,21 @@ __global__ void __launch_bounds__(256) k_copy(const uint8_t* __restrict__ in, ui
 
 // The step's scratch.  alloc(pointer, bytes) -> cudaError_t is the caller's allocator: the memory is the caller's to release.
 template <class Alloc>
-static inline cudaError_t scratch_alloc(StepScratch& s, size_t max_streams, size_t max_bytes, Alloc alloc) {
+static inline cudaError_t scratch_alloc(StepScratch& s, size_t max_streams, Alloc alloc) {
     cudaError_t r;
     if ((r = alloc(s.plan, max_streams * sizeof(SegPlan))) != cudaSuccess) return r;
+    if ((r = cudaMemset(s.plan, 0, max_streams * sizeof(SegPlan))) != cudaSuccess) return r;     // (k_commit2 keeps it zero)
     if ((r = alloc(s.tpl_cache2, sizeof(TemplateCache2))) != cudaSuccess) return r;
     if ((r = cudaMemset(s.tpl_cache2, 0, sizeof(TemplateCache2))) != cudaSuccess) return r;
     if ((r = alloc(s.usage_fields, max_streams * 9 * sizeof(uint2))) != cudaSuccess) return r;
-    if ((r = alloc(s.tile_seg, (max_bytes / R2_TILE + 4) * 4)) != cudaSuccess) return r;
-    if ((r = cudaMemset(s.tile_seg, 0, (max_bytes / R2_TILE + 4) * 4)) != cudaSuccess) return r;
     if ((r = alloc(s.counters, 64)) != cudaSuccess) return r;
     if ((r = cudaMemset(s.counters, 0, 64)) != cudaSuccess) return r;
     if ((r = cudaFuncSetAttribute(k_relay2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)R2_SMEM_BYTES)) != cudaSuccess) return r;
     return cudaSuccess;
 }
 
-// Launch one step on `stream`.  ev[0..3] bracket prime / relay / commit (ev[4] = ev[3]: usage extraction is inside relay and commit).
+// Launch one step on `stream`.  ev[0..3] bracket prime (nothing: ev[1] = ev[0]) / relay / commit (ev[4] = ev[3]: usage extraction is
+// inside relay and commit).
 static inline cudaError_t launch_step(const StepArgs& a, int mode, int sm_count, cudaStream_t stream, cudaEvent_t* ev, int* launched, bool per_kernel) {
     *launched = 0;
     cudaError_t r;

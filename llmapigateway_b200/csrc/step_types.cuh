@@ -12,34 +12,31 @@ struct DeviceTables {
     uint32_t carry_cap, detail_cap, max_streams;
 };
 
+// The bulk path's per-segment record: what k_relay2 found in the segment.  Zero is "nothing found": the scratch is zeroed when
+// it is allocated, and k_commit2 zeroes each segment's record again once it has read it, so every launch set starts from zeros.
+// (The segment's static plan -- bulk region, speculation -- is not stored: SegStatic in relay2.cuh, computed where it is used.)
 struct SegPlan {
-    uint32_t resume_chunk;     // first chunk the sequential path would have to (re)do
-    uint32_t relay_begin;      // byte offset where the bulk region starts (tap view); seg end when none
-    uint32_t seg_end;          // byte offset of the end of the segment
-    uint32_t emit_chunk_begin;
-    uint32_t irregular;        // 1: the bulk kernel's findings are void, k_commit redoes [resume_chunk, end)
+    uint32_t irregular;        // 1: the bulk kernel's findings are void, k_commit2 redoes the segment
     uint32_t a_usage;          // handler bound `tokens_usage` (request_handler.py:134)
     unsigned long long last_usage;   // (1 + byte offset) << 32 | length of the last usage-bearing event (atomicMax)
     uint32_t n_events_a, n_events_b, n_usage_b;
-    // priming by speculation: a fresh stream is assumed to commit on its first non-empty chunk
-    // (request_handler.py:69-95); that chunk's own thread verifies it in the bulk kernel
-    uint32_t kept_chunk;       // 0xFFFFFFFF: no speculation (stream was already committed)
-    uint32_t kept_end;         // byte offset of the end of the kept chunk = where the handler's text starts
     uint32_t prime_ok;         // set by the warp that walks the kept chunk when the speculation holds
-    uint32_t tail_start;       // where the event that is open at the end of the text begins (= new carry); 0xFFFFFFFF: not reached
+    uint32_t tail_start;       // 1 + where the event that is open at the end of the text begins (= new carry); 0: not reached
     uint32_t cand_ps;          // 1 + start of the usage event whose field spans sit in usage_fields[9 * seg ..] (0: none)
 };
-static_assert(sizeof(SegPlan) == 64, "SegPlan");
+static_assert(sizeof(SegPlan) == 40, "SegPlan");
 
 struct TemplateCache2;     // relay2.cuh
 
 struct StepScratch {
-    SegPlan* plan;             // [max_streams]
+    SegPlan* plan;             // [max_streams] what k_relay2 found per segment; all zero between launch sets
+#ifndef __CUDACC__
+    uint32_t* tile_seg;        // host build only, never read: the emulator's step driver (tests/support/host_relay2.cpp) still
+                               //   hands the kernels a tile table, which the device step no longer has
+#endif
     TemplateCache2* tpl_cache2;  // event templates, persistent across steps
     uint2* usage_fields;       // [max_streams][9] a template-following usage event of this step: (start, length | escapes << 31) of its eight
                                //   usage fields as the match located them, [8].x = the template's slot in the engine-wide cache
-    uint32_t* tile_seg;        // [max tiles + 1] segment that holds the first byte of each 3 KiB tile of the launch (tile 0: the
-                               //   launch's first segment with bytes, since its first byte may lie before the launch)
     uint32_t* counters;        // diagnostics since engine creation: [0] segments redone sequentially, [1] segments folded from the bulk
                                //   kernel's findings, [2] usage records read from template spans, [3] usage events stashed
 };
@@ -54,7 +51,7 @@ struct StepArgs {
     const uint32_t* seg_chunk; const uint32_t* seg_slot; uint32_t n_segs;
     uint8_t* out; SegResult* seg_out;
     RowEvent* rowq; uint32_t* rowq_count; uint32_t rowq_cap;
-    uint32_t reset_rows;                       // 1: k_prime2 empties the row queue (the first launch of a step)
+    uint32_t reset_rows;                       // 1: k_relay2 empties the row queue (the first launch of a step)
     StepScratch s;
 };
 

@@ -7,7 +7,7 @@
 //                             the text so far (a "mark": the host cuts the stream's transcript at that position)
 //   chat_logging.py:140-143   any exception skips the rest of the part / the chunk (what was appended stays appended)
 //
-// The relay step (k_prime2 / k_relay2 / k_commit2) decides WHICH chunks are relayed; this pass runs after it over the same
+// The relay step (k_relay2 / k_commit2) decides WHICH chunks are relayed; this pass runs after it over the same
 // packed step (`emit_chunk_begin` of every segment) and is decoupled from the relay state: the tap's buffer is re-derived from
 // the relayed chunks with its own carry, exactly like the reference's tap thread, which sees nothing but the relayed chunks.
 // It is optional (lgw_transcripts_enable): the reference only taps when LOG_CHAT_ENABLED is set (chat_logging.py:166-168).
